@@ -6,6 +6,7 @@ throughput in samples/s, whole job, device timed, max over ranks.
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 \
         --master-port 29500 bench.py --gpus 8 --steps 20 --warmup 5
     python bench.py --impl reference ...        # unmodified reference from baseline/_ref (if installable)
+    python bench.py --dump-outputs DIR ...      # also write the last timed step's outputs as DIR/<name>.npy
 
 Prints ONE JSON line on rank 0 (see README / DESIGN.md for the field contract).
 """
@@ -30,6 +31,8 @@ CRITEO_1TB_40M = [39884406, 39043, 17289, 7420, 20263, 3, 7120, 1543, 63, 385329
                   39979771, 25641295, 39664984, 585935, 12972, 108, 36]
 HOST_HEAD_STEPS = 16  # host enqueue time is averaged over this many steps right after the start barrier
 BASELINE_SAMPLES_PER_SEC = {1: 50_000.0, 8: 350_000.0}  # reference published numbers (A100), BASELINE.md
+RW100M_OTHER_ROW_CAP = 4_000_000
+NVLINK_GBPS = 450.0  # H100 SXM NVLink 4: 18 links, 900 GB/s bidirectional = 450 GB/s per direction (data sheet)
 
 
 def parse_args() -> argparse.Namespace:
@@ -42,7 +45,8 @@ def parse_args() -> argparse.Namespace:
     p.add_argument("--embedding-dim", type=int, default=128)
     p.add_argument("--dense-arch", type=str, default="512,256,128")
     p.add_argument("--over-arch", type=str, default="1024,1024,512,256,1")
-    p.add_argument("--row-cap", type=int, default=int(os.environ.get("TRB_BENCH_ROW_CAP", 40_000_000)))
+    # 20 M rows per table: 49.6 GiB of fp32 tables (+ row-wise Adagrad state) fit one 80 GB H100 beside the batch-32768 activations
+    p.add_argument("--row-cap", type=int, default=int(os.environ.get("TRB_BENCH_ROW_CAP", 20_000_000)))
     p.add_argument("--pooling", type=int, default=1, help="ids per sparse feature (Criteo is one-hot)")
     p.add_argument("--lr", type=float, default=0.01)
     p.add_argument("--config", type=str, default="dlrm", choices=["dlrm", "rw100m", "dcn_cw", "two_tower"],
@@ -59,14 +63,15 @@ def parse_args() -> argparse.Namespace:
     p.add_argument("--dp-rows", type=int, default=int(os.environ.get("TRB_BENCH_DP_ROWS", 0)),
                    help="--sharding table_wise only: tables with at most this many rows are data-parallel when N > 1 (0 = every table model-parallel)")
     p.add_argument("--cuda-graphs", type=int, default=int(os.environ.get("TRB_BENCH_GRAPHS", -1)),
-                   help="1 (= -1, the default): replay the dense sub-modules as CUDA graphs (host enqueue 1.6-2.6 ms -> 0.74 ms per step; "
-                        "end to end 15.4 M -> 17.7 M samples/s on one GPU); 0: eager")
+                   help="1 (= -1, the default): replay the dense sub-modules as CUDA graphs (fewer host launches per step); 0: eager")
     p.add_argument("--profile-host", action="store_true", help="cProfile 10 extra steps on rank 0 (stderr)")
     p.add_argument("--ddp-bucket-mb", type=float, default=float(os.environ.get("TRB_BENCH_DDP_BUCKET_MB", 2)), help="DDP gradient bucket size of the dense part")
     p.add_argument("--no-e2e", action="store_true")
     p.add_argument("--phase-times", action="store_true", help="diagnostics: forward / backward / optimizer device time of the plain step (stderr)")
     p.add_argument("--trace-e2e", type=str, default="", help="diagnostics: torch.profiler trace (chrome json + op table) of 6 extra pipeline steps")
     p.add_argument("--num-host-batches", type=int, default=8)
+    p.add_argument("--dump-outputs", type=str, default="",
+                   help="directory: after the timed steps, write what the last timed step returned (loss, logits, labels) as float32 .npy files")
     return p.parse_args()
 
 
@@ -188,7 +193,9 @@ def build_ours(args: argparse.Namespace, device, rank: int, world: int):
         hashes = [min(h, args.row_cap) for h in CRITEO_1TB_40M]
         keys = [f"cat_{i}" for i in range(26)]
         if cfg == "rw100m":
-            hashes[0] = 100_000_000
+            # the 100 M-row table alone is 51.2 GB of fp32 rows: the other 25 tables are capped at 4 M rows (10.3 GB) so that the
+            # whole config (61.5 GB of fp32 tables) fits one 80 GB H100 beside the batch-32768 activations
+            hashes = [100_000_000] + [min(h, RW100M_OTHER_ROW_CAP) for h in hashes[1:]]
     tables = [EmbeddingBagConfig(name=f"t_{k}", embedding_dim=D, num_embeddings=h, feature_names=[k]) for k, h in zip(keys, hashes)]
     ebc = EmbeddingBagCollection(tables=tables, device=torch.device("meta"))
     apply_optimizer_in_backward(RowWiseAdagrad, ebc.parameters(), {"lr": args.lr, "eps": 1e-8})
@@ -208,10 +215,10 @@ def build_ours(args: argparse.Namespace, device, rank: int, world: int):
 
     backend = args.dense_backend
     if backend == "auto":
-        backend = os.environ.get("TRB_DENSE_DEFAULT", "tcgen05")  # bf16 tensor-core dense path is the product
+        backend = os.environ.get("TRB_DENSE_DEFAULT", "wgmma")  # bf16 tensor-core dense path is the product
     _dense.set_dense_backend(backend)
     # bf16 pooled embeddings (half the NVLink / HBM bytes) when the dense arch computes in bf16
-    fused_params = {"output_dtype": torch.bfloat16} if backend == "tcgen05" else None
+    fused_params = {"output_dtype": torch.bfloat16} if backend == "wgmma" else None
     sharder = EmbeddingBagCollectionSharder(fused_params=fused_params)
 
     # sharding-type constraint of the config (identical rule in the reference arm: baseline/run_reference.py)
@@ -264,8 +271,8 @@ def build_ours(args: argparse.Namespace, device, rank: int, world: int):
     # data-parallel wrapping is deferred (main() calls dmp.init_data_parallel()) so that CUDA graphs of the dense sub-modules can
     # be captured first: DDP keeps the parameters' AccumulateGrad nodes alive on the default stream, which a capture may not touch
     # small DDP buckets: the dense gradients of the top MLP are reduced while the embedding backward + bottom MLP backward still run; with the
-    # default 25 MB cap everything but the last layer waits in ONE bucket for the very last gradient and the all-reduce (239 us at 8 GPUs in
-    # profiles/step_kernels_n8_r2.md) sits exposed at the end of the step
+    # default 25 MB cap everything but the last layer waits in ONE bucket for the very last gradient and the all-reduce sits exposed at the end of
+    # the step
     from torchrec_b200.parallel.model_parallel import DefaultDataParallelWrapper
 
     dmp = DistributedModelParallel(model, device=device, plan=plan, sharders=[sharder], init_data_parallel=False,
@@ -336,7 +343,7 @@ def measure_comm(dmp, device, world: int, iters: int = 10) -> Optional[Dict[str,
     res = {"fwd_fused_lookup_dist_ms": t_fused, "fwd_same_lookup_local_ms": t_local, "bwd_grad_push_ms": t_push, "device_barrier_ms": t_barrier,
            "fwd_sent_bytes_per_rank": sent_fwd, "bwd_sent_bytes_per_rank": sent_bwd,
            "fwd_gbps": sent_fwd / (t_fused * 1e-3) / 1e9, "bwd_gbps": sent_bwd / (max(t_push - t_barrier, 1e-6) * 1e-3) / 1e9,
-           "exposed_fwd_ms": max(0.0, t_fused - t_local), "exposed_bwd_ms": t_push, "nvlink_peak_gbps": 900.0, "nvlink_measured_peer_copy_gbps": 770.0}
+           "exposed_fwd_ms": max(0.0, t_fused - t_local), "exposed_bwd_ms": t_push, "nvlink_peak_gbps": NVLINK_GBPS}
     return res
 
 
@@ -354,7 +361,7 @@ def fp8_inference_qps(args, dmp, device, rank: int, world: int, keys, hashes) ->
     q = QuantTableBatchedEmbeddingBags([(f"t{i}", r, args.embedding_dim, DataType.FP8) for i, r in enumerate(rows)], output_dtype=torch.bfloat16, device=device)
     q.weights.random_(0, 120)  # arbitrary finite e4m3 payloads / scales: the timing does not depend on the values
     g = torch.Generator(device="cpu").manual_seed(7)
-    # 16 distinct batches: 16 x 26 x 32768 rows x 144 B = 1.9 GB of gathered rows, far beyond the 126 MB L2 (no batch is re-read from cache)
+    # 16 distinct batches: 16 x 26 x 32768 rows x 144 B = 1.9 GB of gathered rows, far beyond the 50 MB L2 (no batch is re-read from cache)
     id_sets = [torch.cat([torch.randint(0, r, (B,), generator=g) for r in rows]).to(device) for _ in range(16)]
     off = torch.arange(0, len(rows) * B + 1, device=device, dtype=torch.int64)
     for i in range(4):
@@ -372,7 +379,16 @@ def fp8_inference_qps(args, dmp, device, rank: int, world: int, keys, hashes) ->
     return {"format": "FP8_BLOCK (e4m3, fp16 scale / 32 elems)", "samples_per_s_per_gpu": B / (ms * 1e-3), "ms_per_batch": ms,
             "table_bytes": int(sum(rows)) * row_bytes, "gathered_gbps": len(rows) * B * row_bytes / (ms * 1e-3) / 1e9,
             "hbm_gbps_rows_plus_bf16_output": len(rows) * B * (row_bytes + args.embedding_dim * 2) / (ms * 1e-3) / 1e9,
-            "l2_policy": "16 distinct one-hot batches (1.9 GB of rows) cycled: no batch is served from the 126 MB L2", "out_shape": list(out.shape)}
+            "l2_policy": "16 distinct one-hot batches (1.9 GB of rows) cycled: no batch is served from the 50 MB L2", "out_shape": list(out.shape)}
+
+
+def dump_outputs(out_dir: str, outs) -> None:
+    """The last timed step's (loss, logits, labels) of rank 0 as float32 ``<name>.npy`` (a few hundred KB at batch 32768)."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in zip(("loss", "logits", "labels"), outs):
+        np.save(os.path.join(out_dir, f"{name}.npy"), t.float().reshape(-1).cpu().numpy())
 
 
 def main() -> None:
@@ -411,6 +427,7 @@ def main() -> None:
         os.environ["TRB_TRANSPORT"] = args.transport  # "nccl": the internal UNFUSED arm (own lookup kernels + NCCL all-to-alls)
     _lib.lib()
 
+    torch.manual_seed(0)  # same arguments -> same initial weights and batches, so two builds can be compared output for output
     dmp, opt, keys, hashes, ids_per_feature, num_dense, dense_backend, plan_info = build_ours(args, device, rank, world)
     B = args.batch_size
     ds = RandomRecDataset(keys, B, hash_sizes=hashes, ids_per_features=ids_per_feature, num_dense=num_dense, manual_seed=1234 + rank,
@@ -426,7 +443,7 @@ def main() -> None:
     inner = getattr(dmp.module, "model", None)
     if args.cuda_graphs and hasattr(inner, "capture_dense_graphs"):
         # the dense sub-modules (bottom MLP, interaction + top MLP + head) replay as CUDA graphs: their ~50 launches and ~100 ATen
-        # calls per step made the step launch-bound once DDP / NVLink dists were added (host enqueue 2.0 ms vs 2.1 ms of GPU time)
+        # calls per step make the step launch-bound once DDP / NVLink dists are added (host enqueue time close to the GPU time)
         with torch.no_grad():
             sample_emb = inner.sparse_arch(dev_batches[0].sparse_features)
         inner.capture_dense_graphs(dev_batches[0].dense_features, sample_emb)
@@ -437,12 +454,16 @@ def main() -> None:
         args.cuda_graphs = 0
         dmp.init_data_parallel()
 
-    def step(batch) -> "torch.Tensor":
+    def step(batch, keep: bool = False) -> "torch.Tensor":
         opt.zero_grad()
-        loss, _ = dmp(batch)
+        loss, outs = dmp(batch)
+        if keep:  # the last timed step's outputs: read out after the timed region, before the next forward replays into them
+            kept["outs"] = outs
         loss.backward()
         opt.step()
         return loss
+
+    kept: Dict[str, Any] = {}
 
     def barrier() -> None:
         if world > 1:
@@ -463,7 +484,7 @@ def main() -> None:
     t_host0 = time.perf_counter()
     t_host_head = None
     for i in range(args.steps):
-        loss = step(dev_batches[i % len(dev_batches)])
+        loss = step(dev_batches[i % len(dev_batches)], keep=bool(args.dump_outputs) and i == args.steps - 1)
         if i == HOST_HEAD_STEPS - 1:
             t_host_head = time.perf_counter()
     # CPU time to ENQUEUE a step (>= ms_per_step means launch-bound). Measured over the first steps after the barrier: once the host
@@ -473,6 +494,8 @@ def main() -> None:
     barrier()
     ms = e0.elapsed_time(e1)
     launches = _lib.launch_count() - n0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, kept["outs"])
     if args.phase_times:  # diagnostics: where the device time of the plain step goes (events on the main stream, no profiler attached)
         n_ph = 20
         evs = [[torch.cuda.Event(enable_timing=True) for _ in range(4)] for _ in range(n_ph)]
@@ -621,14 +644,16 @@ def main() -> None:
             "higher_is_better": True,
             "scaling": "weak",
             "vs_baseline": (value / base) if base else None,
-            "dtype": "bf16" if dense_backend == "tcgen05" else "fp32",
+            "dtype": "bf16" if dense_backend == "wgmma" else "fp32",
             "data": "synthetic (random Criteo-1TB-shaped ids/dense, random-init tables)",
             "impl": "ours",
             "config": {
                 "name": args.config,
                 "model": {"dlrm": "DLRM", "rw100m": "DLRM", "dcn_cw": "DLRM-DCNv2 (3 cross layers, rank 512)", "two_tower": "two-tower retrieval (examples/two_tower_retrieval.py)"}[args.config]
                          + " (%d sparse x dim %d, dense %s, over %s), fp32 tables + fused row-wise Adagrad, dense SGD" % (len(keys), args.embedding_dim, args.dense_arch, args.over_arch),
-                "num_embeddings": "%s (%.1f GB fp32 tables)" % ("Criteo-1TB cardinalities capped at %d rows" % args.row_cap if args.config != "two_tower" else str(hashes),
+                "num_embeddings": "%s (%.1f GB fp32 tables)" % (str(hashes) if args.config == "two_tower" else
+                                                                ("t_cat_0: 100 M rows, the other Criteo-1TB cardinalities capped at %d rows" % min(args.row_cap, RW100M_OTHER_ROW_CAP))
+                                                                if args.config == "rw100m" else "Criteo-1TB cardinalities capped at %d rows" % args.row_cap,
                                                                 sum(hashes) * args.embedding_dim * 4 / 1e9),
                 "global_batch": B * world,
                 "per_gpu_batch": B,
@@ -639,7 +664,7 @@ def main() -> None:
                 "transport": ("NVLink sparse plane (fused peer-memory kernels%s)" % (", CUDA-graph phases" if any(p._graphs for p in planes) else "")) if planes else "nccl / local",
                 "overlap_sparse_dense": bool(args.overlap_sparse),
                 "pipeline": "TrainPipelineSparseDist (e2e) / plain step (value)",
-                "l2_policy": "inputs > L2: %d distinct batches, random rows of multi-GB tables (L2 126 MB)" % len(dev_batches),
+                "l2_policy": "inputs > L2: %d distinct batches, random rows of multi-GB tables (L2 50 MB)" % len(dev_batches),
                 "dense_backend": dense_backend,
                 "cuda_graphs": "dense sub-modules (fwd+bwd)" if args.cuda_graphs else "off",
                 "cpu_binding": globals().get("_CPU_BINDING", "off"),
@@ -652,11 +677,11 @@ def main() -> None:
         if e2e is not None:
             out["e2e"] = e2e
         if comm is not None:
-            # BASELINE.json: "exposed all-to-all ms/step; pooled-emb all-to-all GB/s vs 900 GB/s". The input dist is hidden by the pipeline
+            # BASELINE.json: "exposed all-to-all ms/step; pooled-emb all-to-all GB/s vs the NVLink line rate". The input dist is hidden by the pipeline
             # (e2e) and inside the plain step it is part of `comm["input_dist_ms"]`.
             out["exposed_a2a_ms_per_step"] = comm["exposed_fwd_ms"] + comm["exposed_bwd_ms"]
-            out["pooled_a2a_gbps"] = {"fwd_fused_with_lookup": comm["fwd_gbps"], "bwd_grad_push": comm["bwd_gbps"], "line_rate": 900.0,
-                                      "frac_of_900": max(comm["fwd_gbps"], comm["bwd_gbps"]) / 900.0}
+            out["pooled_a2a_gbps"] = {"fwd_fused_with_lookup": comm["fwd_gbps"], "bwd_grad_push": comm["bwd_gbps"], "line_rate": NVLINK_GBPS,
+                                      "frac_of_line_rate": max(comm["fwd_gbps"], comm["bwd_gbps"]) / NVLINK_GBPS}
             out["comm"] = comm
         out.update(extra)
         print(json.dumps(out))

@@ -1,7 +1,7 @@
 """Quantize -> serve (reference examples/inference_legacy, torchrec/inference): build a DLRM, quantize its tables to INT8,
 start the native batching server with a gRPC front end, send requests.
 
-    python examples/inference_server.py            # CPU works too; on a B200 box the executor runs on cuda:0
+    python examples/inference_server.py            # CPU works too; on a GPU box the executor runs on cuda:0
 """
 import os
 import sys

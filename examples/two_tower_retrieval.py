@@ -1,6 +1,6 @@
 """Two-tower retrieval (reference examples/retrieval/two_tower_train.py, modules/two_tower.py): a query tower and a
 candidate tower (EmbeddingBagCollection + MLP each) trained with in-batch softmax; the candidate embeddings are then
-exported and served through brute-force top-k (the reference uses FAISS IVFPQ; here a tcgen05-friendly dense scoring)."""
+exported and served through brute-force top-k (the reference uses FAISS IVFPQ; here a tensor-core-friendly dense scoring)."""
 import os
 import sys
 from typing import List

@@ -1,4 +1,4 @@
-"""The composable per-group kernels / grouped lookups on a B200: CUDA TBE kernels vs the CPU reference path of the same classes."""
+"""The composable per-group kernels / grouped lookups on an H100: CUDA TBE kernels vs the CPU reference path of the same classes."""
 import pytest
 import torch
 

@@ -1,4 +1,4 @@
-"""tcgen05 dot-interaction forward/backward vs the PyTorch formulation (reference dlrm.py:210-222)."""
+"""wgmma dot-interaction forward/backward vs the PyTorch formulation (reference dlrm.py:210-222)."""
 import pytest
 import torch
 
@@ -40,7 +40,7 @@ def test_interaction_fwd_bwd(B, F, sparse_dtype):
     assert float((sparse.grad.float() - s32.grad).abs().max()) < tol_s
 
 
-def test_dlrm_with_tcgen05_backend_matches_torch():
+def test_dlrm_with_wgmma_backend_matches_torch():
     from torchrec_b200.models.dlrm import DLRM
     from torchrec_b200.modules.embedding_configs import EmbeddingBagConfig
     from torchrec_b200.modules.embedding_modules import EmbeddingBagCollection
@@ -59,7 +59,7 @@ def test_dlrm_with_tcgen05_backend_matches_torch():
     ref.sum().backward()
     gref = {n: p.grad.clone() for n, p in m.named_parameters() if p.grad is not None}
     m.zero_grad()
-    D.set_dense_backend("tcgen05")
+    D.set_dense_backend("wgmma")
     try:
         out = m(x, kjt)
         out.sum().backward()
@@ -83,7 +83,7 @@ def test_dlrm_dense_cuda_graphs_match_eager():
     from torchrec_b200.ops import dense as _dense
 
     dev = torch.device("cuda:0")
-    _dense.set_dense_backend("tcgen05")
+    _dense.set_dense_backend("wgmma")
     try:
         keys = [f"f{i}" for i in range(26)]
 

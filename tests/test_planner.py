@@ -148,7 +148,7 @@ def test_annotation_estimator_and_shard_estimators():
     assert get_embedding_perf_sharding_evaluator("row_wise", cfg).evaluate(ctx("row_wise", n_row=8)).fwd_compute == 123.0
     with pytest.raises(PlannerError):
         get_embedding_perf_sharding_evaluator("grid_shard", cfg)
-    assert EmbeddingPerfEstimatorFactory.available() == ["b200", "gb200"]
+    assert EmbeddingPerfEstimatorFactory.available() == ["gb200", "h100"]
     assert EmbeddingPerfEstimatorFactory.get_config("gb200").hbm_to_ddr_mem_bw > K.HBM_TO_DDR_MEM_BW
 
     # functional storage helpers
@@ -167,14 +167,16 @@ def test_annotation_estimator_and_shard_estimators():
 
 
 def test_perf_model_matches_measured_fused_kernels():
-    """The planner's table-wise costs for the DLRM headline plan against what the kernels measured on 8 x B200 (profiles/scaling_r2.md):
-    fused lookup + output dist 0.490 ms (lookup alone 0.135 ms) on the rank with 4 tables at W = 8, 0.176 ms / 0.110 ms at W = 2."""
+    """The planner's table-wise lookup costs for the DLRM headline plan against what the kernels measured on one H100 80GB HBM3
+    (``tools/kernel_bench.py``, the busiest rank of the W = 8 job: 4 tables x 262144 one-hot samples, fp32 rows -> bf16, row-wise
+    Adagrad): forward 0.297 ms, backward 0.776 ms. The NVLink half (fused lookup + output dist) needs 8 GPUs to measure and is not
+    asserted."""
     import torch
 
     from torchrec_b200.modules.embedding_configs import EmbeddingBagConfig
     from torchrec_b200.modules.embedding_modules import EmbeddingBagCollection
     from torchrec_b200.parallel.embeddingbag import EmbeddingBagCollectionSharder
-    from torchrec_b200.parallel.planner import EmbeddingShardingPlanner, Topology, calibration
+    from torchrec_b200.parallel.planner import EmbeddingShardingPlanner, Topology
     from torchrec_b200.parallel.planner.types import ParameterConstraints
 
     hashes = [39884406, 39043, 17289, 7420, 20263, 3, 7120, 1543, 63, 38532951, 2953546, 403346, 10, 2208, 11938, 155, 4, 976, 14, 39979771, 25641295, 39664984,
@@ -186,22 +188,21 @@ def test_perf_model_matches_measured_fused_kernels():
             super().__init__()
             self.ebc = EmbeddingBagCollection(tables=tables, device=torch.device("meta"))
 
-    measured = {2: (0.110, 0.176), 8: (0.135, 0.490)}
-    for W, (lookup_ms, fused_ms) in measured.items():
-        planner = EmbeddingShardingPlanner(topology=Topology(world_size=W, local_world_size=W, compute_device="cuda"), batch_size=32768,
-                                           constraints={t.name: ParameterConstraints(sharding_types=["table_wise"], compute_kernels=["fused"]) for t in tables})
-        planner.plan(M(), [EmbeddingBagCollectionSharder(fused_params={"output_dtype": torch.bfloat16})])
-        per = {}
-        for so in planner._best_plan:
-            for sh in so.shards:
-                d = per.setdefault(sh.rank, [0.0, 0.0])
-                d[0] += sh.perf.fwd_compute
-                d[1] += sh.perf.fwd_comms
-        fc, fm = max(per.values(), key=lambda d: d[0] + d[1])
-        assert fc == pytest.approx(lookup_ms, rel=0.35), (W, fc, lookup_ms)
-        assert fc + fm == pytest.approx(fused_ms, rel=0.25), (W, fc + fm, fused_ms)
-    assert calibration.all_to_all_gbps(8) < calibration.all_to_all_gbps(2) < calibration.PEER_STORE_GBPS
-    assert calibration.all_to_all_gbps(4) == pytest.approx(670 * 0.85)
+    W, fwd_ms, bwd_ms = 8, 0.297, 0.776
+    planner = EmbeddingShardingPlanner(topology=Topology(world_size=W, local_world_size=W, compute_device="cuda"), batch_size=32768,
+                                       constraints={t.name: ParameterConstraints(sharding_types=["table_wise"], compute_kernels=["fused"]) for t in tables})
+    planner.plan(M(), [EmbeddingBagCollectionSharder(fused_params={"output_dtype": torch.bfloat16})])
+    per = {}
+    for so in planner._best_plan:
+        for sh in so.shards:
+            d = per.setdefault(sh.rank, [0.0, 0.0, 0])
+            d[0] += sh.perf.fwd_compute
+            d[1] += sh.perf.bwd_compute
+            d[2] += 1
+    fc, bc, n_tables = max(per.values(), key=lambda d: d[0])
+    assert n_tables == 4, per  # the measured shape: the busiest rank looks up 4 tables for the global batch
+    assert fc == pytest.approx(fwd_ms, rel=0.25), (fc, fwd_ms)
+    assert bc == pytest.approx(bwd_ms, rel=0.25), (bc, bwd_ms)
 
 
 def test_plan_loader_topology_factory_and_planner_helpers():
@@ -282,10 +283,10 @@ def test_plan_loader_topology_factory_and_planner_helpers():
         validate_modules_inclusion_in_sharding_plan(ShardingPlan({}), Model(), sharders)
     assert e.value.error_type == PlannerErrorType.MISSING_MODULE_IN_PLAN
     # topology from layers: trainer > hardware > defaults; dry run; bandwidths only from hardware when asked
-    hw = HardwareConfig(hbm_cap_bytes=180 * 2**30, ddr_cap_bytes=2**40, intra_host_bw=7.0, hbm_mem_bw=9.0, additional_params={"gen": "b200"})
+    hw = HardwareConfig(hbm_cap_bytes=180 * 2**30, ddr_cap_bytes=2**40, intra_host_bw=7.0, hbm_mem_bw=9.0, additional_params={"gen": "h100"})
     t = TopologyFactory.create_topology(TrainerConfig(world_size=16, local_world_size=8, hbm_cap_bytes=100 * 2**30), hw, KernelConfig(use_hardware_based_bandwidth=True))
     assert (t.world_size, t.local_world_size, t.devices[3].storage.hbm, t.devices[3].storage.ddr) == (16, 8, 100 * 2**30, 2**40)
-    assert t.comms_bandwidths.intra_host_bw == 7.0 and t.hbm_mem_bw == 9.0 and hw.get_param("gen") == "b200" and not hw.has_param("x")
+    assert t.comms_bandwidths.intra_host_bw == 7.0 and t.hbm_mem_bw == 9.0 and hw.get_param("gen") == "h100" and not hw.has_param("x")
     t2 = TopologyFactory.create_topology(TrainerConfig(world_size=2, is_dry_run=True, dry_run_hbm_bytes=5 * 2**30), hw)
     assert t2.devices[0].storage.hbm == 5 * 2**30 and t2.comms_bandwidths.intra_host_bw != 7.0
     with pytest.raises(ValueError):

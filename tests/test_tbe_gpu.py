@@ -1,4 +1,4 @@
-"""Numerics of the sm_100a TBE kernels vs the fp32 PyTorch reference implementation."""
+"""Numerics of the sm_90a TBE kernels vs the fp32 PyTorch reference implementation."""
 import pytest
 import torch
 

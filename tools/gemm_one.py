@@ -1,4 +1,4 @@
-"""Run ONE GEMM shape a few times (target for `ncu -k regex:gemm_bf16_tcgen05 --launch-skip 2 -c 1`).
+"""Run ONE GEMM shape a few times (target for `ncu -k regex:gemm_bf16_wgmma --launch-skip 2 -c 1`).
 Usage: python tools/gemm_one.py M N K [tile_n] [mode: 0 plain, 1 bias+relu, 2 masked dgrad]"""
 import os
 import sys

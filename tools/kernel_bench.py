@@ -4,14 +4,12 @@
 Every peer kernel runs in loopback (W virtual ranks, all symmetric buffers on this device), so the numbers are the HBM side of the
 kernels; the NVLink side is `tools/peer_bench.py` (2 GPUs, one process) and `bench.py --measure-comm` (N processes).
 For each case: device time (CUDA events, L2 flushed before every iteration, median), the bytes the kernel has to move by its own
-definition (compulsory traffic), GB/s, and the fraction of the MEASURED copy bandwidth in MEASURED_PEAKS.json (`hbm_gbs`).
+definition (compulsory traffic), GB/s, and the fraction of the device-to-device copy bandwidth measured at start-up on this GPU.
 
-    python tools/kernel_bench.py [--batch 32768] [--iters 15] [--only tbe_fwd] [--md profiles/kernel_roofline_r2.md]
-    ncu --set full --clock-control none --import-source on -k regex:'tbe_|kjt_|trb_|qtbe' -c 40 -o gpurun_out/ncu_kernels_r2 \
-        python tools/kernel_bench.py --iters 1 --no-flush
+    python tools/kernel_bench.py [--batch 32768] [--iters 15] [--only tbe_fwd] [--md kernel_roofline.md]
 """
 import argparse
-import json
+import gc
 import os
 import sys
 
@@ -34,11 +32,23 @@ CRITEO = [39884406, 39043, 17289, 7420, 20263, 3, 7120, 1543, 63, 38532951, 2953
           39979771, 25641295, 39664984, 585935, 12972, 108, 36]
 
 
-def peaks() -> float:
-    try:
-        return float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"])
-    except Exception:
-        return 6588.7
+def copy_gbs(dev: torch.device, nbytes: int = 2 << 30, iters: int = 10) -> float:
+    """Device-to-device copy bandwidth (read + write bytes per second), median of ``iters`` CUDA-event timed copies."""
+    src = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    dst = torch.empty_like(src)
+    for _ in range(3):
+        dst.copy_(src)
+    ts = []
+    for _ in range(iters):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        dst.copy_(src)
+        e1.record()
+        torch.cuda.synchronize()
+        ts.append(e0.elapsed_time(e1) * 1e-3)
+    del src, dst
+    torch.cuda.empty_cache()
+    return 2.0 * nbytes / sorted(ts)[len(ts) // 2] / 1e9
 
 
 class Bench:
@@ -47,7 +57,8 @@ class Bench:
         self.dev = torch.device("cuda:0")
         self.flush = None if a.no_flush else torch.empty(256 << 20, dtype=torch.uint8, device=self.dev)
         self.rows = []
-        self.hbm = peaks()
+        self.hbm = copy_gbs(self.dev)
+        print(f"{torch.cuda.get_device_name(self.dev)}: device-to-device copy {self.hbm:.0f} GB/s", flush=True)
 
     def run(self, name: str, fn, nbytes: float, note: str = "") -> None:
         if self.a.only and self.a.only not in name:
@@ -154,7 +165,7 @@ def n8_rank_cases(bn: Bench) -> None:
     pl = ids.plane
     reg = pl.regions(ids.slot)
     isz = vals.element_size()
-    bn.run("N=8 busiest rank: tbe_pooled_fwd (4 x 40M-row tables, 262144 samples)", lambda: pl._forward_kernels(reg, 0), N * D * (4 + 2) + N * isz,
+    bn.run(f"N=8 busiest rank: tbe_pooled_fwd (4 x {rows[0] // 1_000_000}M-row tables, {B} samples)", lambda: pl._forward_kernels(reg, 0), N * D * (4 + 2) + N * isz,
            f"{N} rows x 512 B gathered")
     grad = torch.randn(B, F * D, device=dev).to(torch.bfloat16)
     pl._backward_kernels(reg, ids.slot, 1.0, phase=1)
@@ -222,7 +233,7 @@ def jagged_cases(bn: Bench) -> None:
 def main() -> None:
     ap = argparse.ArgumentParser()
     ap.add_argument("--batch", type=int, default=32768)
-    ap.add_argument("--row-cap", type=int, default=40_000_000)
+    ap.add_argument("--row-cap", type=int, default=20_000_000)
     ap.add_argument("--iters", type=int, default=15)
     ap.add_argument("--only", type=str, default="")
     ap.add_argument("--no-flush", action="store_true")
@@ -242,10 +253,11 @@ def main() -> None:
 
             traceback.print_exc()
             print(f"[{nm}] failed: {e}", flush=True)
+        gc.collect()  # the engines of a family hold reference cycles: free their tables before the next family allocates
         torch.cuda.empty_cache()
     if a.md:
         with open(a.md, "w") as f:
-            f.write(f"| kernel (DLRM shapes, batch {a.batch}, 26 x dim 128) | us | compulsory MB | GB/s | % of measured copy bw ({bn.hbm:.0f} GB/s) | bytes counted |\n|---|---|---|---|---|---|\n")
+            f.write(f"| kernel (DLRM shapes, batch {a.batch}, 26 x dim 128) | us | compulsory MB | GB/s | % of measured copy bw ({bn.hbm:.0f} GB/s, {torch.cuda.get_device_name(bn.dev)}) | bytes counted |\n|---|---|---|---|---|---|\n")
             for name, us, mb, gbs, pct, note in bn.rows:
                 f.write(f"| `{name}` | {us:.1f} | {mb:.1f} | {gbs:.0f} | {pct:.1f} | {note} |\n")
 

@@ -1,5 +1,5 @@
-"""Per-op micro-benchmarks on one B200 (CUDA events, L2 flushed between iterations, median of N).
-Usage: python tools/microbench.py [gemm] [interaction] [tbe]   -> prints a markdown table (copied into profiles/)."""
+"""Per-op micro-benchmarks on one H100 (CUDA events, L2 flushed between iterations, median of N).
+Usage: python tools/microbench.py [gemm] [interaction] [tbe]   -> prints markdown tables."""
 import os
 import sys
 
@@ -48,14 +48,14 @@ def bench_gemm():
         if K % 8 == 0 and K >= 64:
             us = timeit(lambda: G.gemm_bf16(gy, wt, b_mn=True))
             print(f"| {M},{K},{N} | dgrad (B MN-major) | {us:.1f} | {2 * M * N * K / us / 1e6:.0f} |")
-            sp, tn = G._wgrad_plan(N, a.shape[1], M, 148)
+            sp, tn = G._wgrad_plan(N, a.shape[1], M, torch.cuda.get_device_properties(dev).multi_processor_count)
             us = timeit(lambda: G.gemm_bf16(gy, a, a_mn=True, b_mn=True, out_dtype=torch.float32, split_k=sp, tile_n=tn))
             print(f"| {N},{K},{M} | wgrad (A,B MN-major, split-K {sp}, tile_n {tn}) | {us:.1f} | {2 * M * N * K / us / 1e6:.0f} |")
 
 
 def bench_gemmx():
-    """Mainloop vs epilogue: sweep K at fixed M, N for the 128 x 256 (tile_n=256) and CTA-pair (tile_n=512) kernels."""
-    print("| M,N,K | variant | tile 128x256 us (TF/s) | pair 256x256 us (TF/s) |\n|---|---|---|---|")
+    """Mainloop vs epilogue: sweep K at fixed M, N."""
+    print("| M,N,K | variant | us | TFLOP/s |\n|---|---|---|---|")
     M, N = 32768, 1024
     for K in (512, 1024, 2048, 4096):
         a = torch.randn(M, K, device=dev).bfloat16()
@@ -65,16 +65,13 @@ def bench_gemmx():
         out = torch.empty(M, N, device=dev, dtype=torch.bfloat16)
         mask = torch.randn(M, N, device=dev).bfloat16()
         for name, fn in [
-            ("K-major B, bias+relu", lambda tn: G.gemm_bf16(a, w, bias=bias, act=G.ACT_RELU, out=out, tile_n=tn)),
-            ("K-major B, plain", lambda tn: G.gemm_bf16(a, w, out=out, tile_n=tn)),
-            ("MN-major B, plain", lambda tn: G.gemm_bf16(a, wt, b_mn=True, out=out, tile_n=tn)),
-            ("MN-major B, relu-grad mask", lambda tn: G.gemm_bf16(a, wt, b_mn=True, out=out, act=G.ACT_RELU_GRAD, mask=mask, tile_n=tn)),
+            ("K-major B, bias+relu", lambda: G.gemm_bf16(a, w, bias=bias, act=G.ACT_RELU, out=out)),
+            ("K-major B, plain", lambda: G.gemm_bf16(a, w, out=out)),
+            ("MN-major B, plain", lambda: G.gemm_bf16(a, wt, b_mn=True, out=out)),
+            ("MN-major B, relu-grad mask", lambda: G.gemm_bf16(a, wt, b_mn=True, out=out, act=G.ACT_RELU_GRAD, mask=mask)),
         ]:
-            r = []
-            for tn in (256, 512):
-                us = timeit(lambda: fn(tn))
-                r.append(f"{us:.1f} ({2 * M * N * K / us / 1e6:.0f})")
-            print(f"| {M},{N},{K} | {name} | {r[0]} | {r[1]} |")
+            us = timeit(fn)
+            print(f"| {M},{N},{K} | {name} | {us:.1f} | {2 * M * N * K / us / 1e6:.0f} |")
 
 
 def bench_colsum():
@@ -128,7 +125,7 @@ def bench_tbe(rows_per_table=40_000_000, n_tables=8):
 
 if __name__ == "__main__":
     which = sys.argv[1:] or ["gemm", "interaction", "tbe"]
-    print(f"env: TRB_GEMM_WIDE={os.environ.get('TRB_GEMM_WIDE')} TRB_INTERACTION_LEGACY={os.environ.get('TRB_INTERACTION_LEGACY')}\n")
+    print(f"env: TRB_INTERACTION_LEGACY={os.environ.get('TRB_INTERACTION_LEGACY')}\n")
     for w in which:
         {"gemm": bench_gemm, "interaction": bench_interaction, "tbe": bench_tbe, "colsum": bench_colsum, "gemmx": bench_gemmx}[w]()
         print()

@@ -1,4 +1,4 @@
-"""torchrec_b200 - a B200-native (sm_100a) recommender-systems framework with the capabilities of TorchRec.
+"""torchrec_b200 - an H100-native (sm_90a) recommender-systems framework with the capabilities of TorchRec.
 
 Top-level surface mirrors ``torchrec/__init__.py``: sparse types, embedding configs / modules, the distributed runtime (``torchrec_b200.distributed`` ==
 ``torchrec_b200.parallel``), quantization and the FX tracer. The CUDA extensions under ``ops/`` are built in-tree by ``__graft_entry__.build()`` and are

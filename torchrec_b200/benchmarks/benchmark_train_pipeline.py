@@ -5,7 +5,7 @@
 
 Config keys (all optional): model {name: dlrm|deepfm, dense_arch, over_arch, embedding_dim}, tables {num, rows, pooling},
 run {batch_size, steps, warmup, pipelines: [base, sparse_dist, sparse_dist_lite, fused_sparse_dist, semi_sync, prefetch],
-sharding: table_wise|row_wise|column_wise|planner, dense_backend: torch|tcgen05}. Prints one JSON line per pipeline."""
+sharding: table_wise|row_wise|column_wise|planner, dense_backend: torch|wgmma}. Prints one JSON line per pipeline."""
 from __future__ import annotations
 
 import argparse

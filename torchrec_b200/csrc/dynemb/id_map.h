@@ -1,6 +1,6 @@
 // Dynamic-embedding id transformer: global id -> cache slot with LFU/LRU eviction metadata.
 //
-// B200-first host design (the table lives in 180 GB HBM; the host only has to keep up with the KJT rate):
+// GPU-first host design (the table lives in HBM; the host only has to keep up with the KJT rate):
 //  * flat open-addressing hash map (linear probing, tombstone-free backward-shift delete), 24 B / entry, one cache
 //    line per probe on average — instead of the node-based std::unordered_map of the reference
 //    (torchrec/csrc/dynamic_embedding/details/naive_id_transformer_impl.h);

@@ -2,7 +2,7 @@
 //
 // An IO backend stores rows (opaque byte blobs) keyed by (table, column-group, global id). Backends are looked up by
 // URL scheme in a process-wide registry: built in are `memory://<name>` (shared in-process store: the DDR tier of a
-// 180 GB-HBM cache, and the test double) and `file://<dir>` (append-only log + in-memory index, survives restarts).
+// HBM cache, and the test double) and `file://<dir>` (append-only log + in-memory index, survives restarts).
 // External plugins (`.so` exporting `trb_io_plugin`) can be loaded at runtime, mirroring the reference's redis plugin
 // (torchrec/csrc/dynamic_embedding/details/io_registry.h, io.h, redis/).
 #pragma once

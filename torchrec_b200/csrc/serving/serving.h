@@ -3,7 +3,7 @@
 //
 // Parity: reference torchrec/inference(_legacy): BatchingQueue (BatchingQueue.h/.cpp), Batching.cpp (dense / sparse
 // combine), GPUExecutor + ResourceManager (outstanding-batch limits), ResultSplit.cpp, Observer.h. Re-designed around
-// B200 serving: the batcher writes ONE contiguous pinned slab per batch (dense | lengths | values | weights...) so the
+// GPU serving: the batcher writes ONE contiguous pinned slab per batch (dense | lengths | values | weights...) so the
 // executor issues a single H2D copy per batch, and sparse features are merged straight into the key-major KJT layout the
 // embedding kernels consume (no per-feature tensors, no second permute on the device).
 #pragma once

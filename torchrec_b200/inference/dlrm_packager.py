@@ -27,7 +27,7 @@ def parse_args(argv: List[str]) -> argparse.Namespace:
     p.add_argument("--embedding_dim", type=int, default=64)
     p.add_argument("--num_dense_features", type=int, default=len(DEFAULT_INT_NAMES))
     p.add_argument("--weight_dtype", type=str, default="INT8", choices=[d.value for d in (DataType.FP32, DataType.FP16, DataType.BF16, DataType.INT8, DataType.INT4, DataType.FP8)],
-                   help="row format of the quantized tables (FP8 = block-scaled e4m3, the B200-native serving format)")
+                   help="row format of the quantized tables (FP8 = block-scaled e4m3)")
     p.add_argument("--sample_batch_size", type=int, default=2, help="rows of the sample input stored with the package")
     p.add_argument("--output_path", type=str, required=True)
     return p.parse_args(argv)

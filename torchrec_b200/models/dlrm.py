@@ -3,8 +3,8 @@
 Architecture parity with the reference (torchrec/models/dlrm.py:38-960): SparseArch (EBC ->
 [B, F, D]), DenseArch (bottom MLP), InteractionArch (pairwise dots) / InteractionDCNArch
 (low-rank cross net) / InteractionProjectionArch, OverArch (top MLP, last layer linear).
-Dense compute is routed through ``torchrec_b200.ops.dense`` so that on B200 the MLP layers and
-the dot interaction run as hand-written tcgen05 kernels.
+Dense compute is routed through ``torchrec_b200.ops.dense`` so that on an H100 the MLP layers and
+the dot interaction run as hand-written wgmma kernels.
 """
 from __future__ import annotations
 
@@ -137,7 +137,7 @@ class OverArch(nn.Module):
             from ..ops import dense as _dense
             from ..ops import head as _head
 
-            if _dense.get_dense_backend() == "tcgen05" and _head.rowdot_supported(hidden, last.weight):
+            if _dense.get_dense_backend() == "wgmma" and _head.rowdot_supported(hidden, last.weight):
                 return _head.RowDotFn.apply(hidden, last.weight, last.bias)  # fused logit layer (+ ReLU mask of `hidden` in its dgrad)
         if hidden.dtype != last.weight.dtype:  # bf16 activations from the fused kernels -> fp32 logits
             hidden = hidden.to(last.weight.dtype)
@@ -186,8 +186,7 @@ class DLRM(nn.Module):
     def capture_dense_graphs(self, sample_dense_features: torch.Tensor, sample_embedded_sparse: torch.Tensor, num_warmup_iters: int = 3) -> None:
         """Capture forward AND backward of the bottom MLP and of interaction + top MLP into CUDA graphs
         (``torch.cuda.make_graphed_callables``). The dense part of a DLRM step is ~50 small launches + ~100 ATen calls whose
-        *enqueue* time (2.0 ms on the host) matched the GPU time of the whole step on B200 (2.1 ms): with more ranks (DDP, NVLink
-        dists) the step became launch-bound. Replaying two graphs removes that host time; the sparse part stays eager, so jagged
+        *enqueue* time can match the GPU time of the whole step: with more ranks (DDP, NVLink dists) the step becomes launch-bound. Replaying two graphs removes that host time; the sparse part stays eager, so jagged
         inputs keep their dynamic shapes. Batches whose shapes differ from the samples fall back to the eager modules.
 
         Call it BEFORE the dense part is wrapped in DDP (``DistributedModelParallel(..., init_data_parallel=False)``, capture, then
@@ -235,7 +234,7 @@ class DLRM(nn.Module):
         s_es = sample_embedded_sparse.detach().clone().requires_grad_()
         if plane is not None and sample_embedded_sparse.numel() == plane.B_local * plane.total_cols and sample_embedded_sparse.dtype == plane.wire_dtype:
             # the embedding arch's TRAINING output always lands in slot 0 of the plane's symmetric buffer: make that memory the graph's
-            # static input, so that the per-step copy of the [B, F * D] embeddings into the graph (73 us on B200) disappears
+            # static input, so that the per-step copy of the [B, F * D] embeddings into the graph disappears
             s_es = plane.out_local(0).view(sample_embedded_sparse.shape).requires_grad_()
         inter_over = _InterOver(self.inter_arch, self.over_arch)
         # capture on a HIGH-priority stream: the captured nodes inherit it, the deferred weight-gradient kernels (side stream, default

@@ -85,16 +85,16 @@ class LowRankCrossNet(nn.Module):
         self.bias: nn.ParameterList = nn.ParameterList(
             [nn.Parameter(nn.init.zeros_(torch.empty(in_features))) for _ in range(num_layers)])
 
-    def _tcgen05_ok(self, x: torch.Tensor) -> bool:
+    def _wgmma_ok(self, x: torch.Tensor) -> bool:
         from ..ops import dense as _dense
 
-        return (_dense.get_dense_backend() == "tcgen05" and x.is_cuda and x.dim() == 2 and x.shape[1] % 8 == 0 and self._low_rank % 8 == 0)
+        return (_dense.get_dense_backend() == "wgmma" and x.is_cuda and x.dim() == 2 and x.shape[1] % 8 == 0 and self._low_rank % 8 == 0)
 
     def forward(self, input: torch.Tensor) -> torch.Tensor:
         x_0 = input
         x_l = x_0
-        if self._tcgen05_ok(input):
-            # both projections on the hand-written sm_100a GEMM (bf16 operands, fp32 accumulation in TMEM, bias fused in the
+        if self._wgmma_ok(input):
+            # both projections on the hand-written sm_90a GEMM (bf16 operands, fp32 accumulation in registers, bias fused in the
             # epilogue of the second one); the Hadamard + residual stay element-wise in the activation dtype
             from ..ops import dense as _dense
 

@@ -1,8 +1,8 @@
 """Perceptron / MLP (reference torchrec/modules/mlp.py:18-190).
 
 On CUDA with bf16/fp16 compute enabled (``torchrec_b200.ops.dense.set_dense_backend``) a
-``Linear + bias + ReLU`` layer runs as ONE hand-written tcgen05/TMEM GEMM kernel with the bias
-and activation fused into the epilogue (``csrc/gemm_tcgen05.cu``); otherwise plain PyTorch.
+``Linear + bias + ReLU`` layer runs as ONE hand-written wgmma GEMM kernel with the bias
+and activation fused into the epilogue (``csrc/gemm_wgmma.cu``); otherwise plain PyTorch.
 """
 from typing import Callable, List, Optional, Union
 
@@ -86,7 +86,7 @@ class MLP(nn.Module):
     def forward(self, input: torch.Tensor) -> torch.Tensor:
         layers = list(self._mlp)
         if input.is_cuda and input.dim() == 2 and len(layers) > 1 and all(isinstance(l, Perceptron) and _dense.fused_act_code(l._activation_fn) is not None for l in layers):
-            # tcgen05 path: the bf16 operands of every layer come from ONE cast kernel in front of the stack
+            # wgmma path: the bf16 operands of every layer come from ONE cast kernel in front of the stack
             wbs = _dense.cast_weights_once([l._linear for l in layers])
             if wbs is not None:
                 x = input

@@ -1,4 +1,4 @@
-"""ctypes loader for the sm_100a kernel library (``torchrec_b200/ops/_lib/libtrb200_ops.so``).
+"""ctypes loader for the sm_90a kernel library (``torchrec_b200/ops/_lib/libtrb200_ops.so``).
 
 The CUDA path is the product: on a machine with a GPU a missing / unloadable library raises
 immediately (no silent PyTorch fallback). On a CPU-only machine every op runs its PyTorch
@@ -52,7 +52,7 @@ def _load() -> Optional[ctypes.CDLL]:
                 _build.build()
             except Exception as e:  # pragma: no cover - depends on toolchain
                 if torch.cuda.is_available():
-                    raise KernelLibraryError(f"cannot build the sm_100a kernel library: {e}") from e
+                    raise KernelLibraryError(f"cannot build the sm_90a kernel library: {e}") from e
         if os.path.exists(path):
             try:
                 _LIB = ctypes.CDLL(path, mode=ctypes.RTLD_GLOBAL)

@@ -1,9 +1,9 @@
-"""In-tree build of the sm_100a kernel library (plain nvcc, C ABI, loaded with ctypes).
+"""In-tree build of the sm_90a kernel library (plain nvcc, C ABI, loaded with ctypes).
 
 ``python -m torchrec_b200.ops.build`` (or ``__graft_entry__.build()``) compiles every ``csrc/*.cu``
-with ``-gencode arch=compute_100a,code=sm_100a -lineinfo`` into ``torchrec_b200/ops/_lib/``.
-Objects are rebuilt only when a source or header is newer. The shared objects are git-ignored
-but travel to the GPU box with the repo snapshot.
+with ``-gencode arch=compute_90a,code=sm_90a -lineinfo`` into ``torchrec_b200/ops/_lib/``.
+Objects are rebuilt only when a source or header is newer; objects, compiler logs and the shared
+object are build products (git-ignored).
 """
 from __future__ import annotations
 
@@ -20,7 +20,7 @@ OUT = os.path.join(HERE, "_lib")
 LIB_NAME = "libtrb200_ops.so"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden",
     "-Xptxas", "-v",
@@ -79,7 +79,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
             list(ex.map(lambda so: _compile_one(so[0], so[1], verbose), todo))
     lib = lib_path()
     if todo or not os.path.exists(lib) or any(os.path.getmtime(o) > os.path.getmtime(lib) for o in objs):
-        cmd = [_nvcc(), "-shared", "-o", lib + ".tmp", *objs, "-gencode", "arch=compute_100a,code=sm_100a",
+        cmd = [_nvcc(), "-shared", "-o", lib + ".tmp", *objs, "-gencode", "arch=compute_90a,code=sm_90a",
                "-Xcompiler", "-fPIC"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:

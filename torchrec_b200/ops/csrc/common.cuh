@@ -1,4 +1,4 @@
-// Common helpers for the torchrec_b200 sm_100a kernel library.
+// Common helpers for the torchrec_b200 sm_90a kernel library.
 //
 // The library is a plain C ABI (.so loaded with ctypes): every entry point takes raw device
 // pointers + a cudaStream_t, so it builds in seconds with nvcc alone (no torch headers) and the
@@ -20,6 +20,14 @@ enum TrbDType : int { TRB_F32 = 0, TRB_F16 = 1, TRB_BF16 = 2, TRB_U8 = 3, TRB_I3
 struct TrbPeerPtrs {
   void* p[TRB_MAX_PEERS];
 };
+
+// SM count of the current device: grid size of the persistent / grid-stride kernels
+inline int trb_num_sms() {
+  int dev = 0, sms = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  return sms > 0 ? sms : 1;
+}
 
 // ---- launch accounting ------------------------------------------------------------------
 // Every kernel launch of this library bumps a host-side counter so bench.py can report

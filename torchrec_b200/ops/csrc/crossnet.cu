@@ -1,6 +1,6 @@
 // Element-wise halves of the DCN-v2 cross layer  x_{l+1} = x_0 * u + x_l  (u = W_l (V_l x_l) + b_l comes out of the GEMM epilogue).
 // In eager PyTorch the forward is 2 kernels over [B, D] bf16 tensors and the backward 4-6 more (mul, mul, add-into-grad ...): for the
-// 3-layer, 3456-wide cross net of the DLRM-DCN benchmark that was ~1.7 ms per step of pure HBM streaming. Here:
+// 3-layer, 3456-wide cross net of the DLRM-DCN benchmark that is a large share of the step, all HBM streaming. Here:
 //   forward   y = x0 * u + xl                                   (3 reads, 1 write)
 //   backward  gu = g * x0;  gx0 = g * u                         (3 reads, 2 writes; the gradient of xl is g itself, no kernel)
 // bf16 storage, fp32 math, 16-byte vectors, grid-stride.
@@ -61,7 +61,8 @@ __global__ void __launch_bounds__(256) cross_bwd_kernel(const uint4* __restrict_
 
 unsigned grid_for(int64_t nvec) {
   const int64_t b = (nvec + 255) / 256;
-  return (unsigned) (b < 148 * 8 ? b : 148 * 8);
+  const int64_t cap = (int64_t) trb_num_sms() * 8;
+  return (unsigned) (b < cap ? b : cap);
 }
 
 }  // namespace

@@ -1,4 +1,4 @@
-// Fused model head for binary CTR models (sm_100a): the final Linear(K -> 1) and BCE-with-logits (mean) loss.
+// Fused model head for binary CTR models (sm_90a): the final Linear(K -> 1) and BCE-with-logits (mean) loss.
 //
 // In the reference the DLRM head is ~25 small library kernels per step (bf16->fp32 cast, gemv, sigmoid / log-sigmoid /
 // mul / add / mean for the loss, their backward twins, split-K gemv for the weight gradient, ReLU mask of the last hidden

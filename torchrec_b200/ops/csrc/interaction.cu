@@ -1,23 +1,23 @@
-// DLRM dot-interaction forward / backward on tcgen05 tensor cores (sm_100a).
+// DLRM dot-interaction forward / backward on wgmma tensor cores (sm_90a).
 //
 //   X_b = [dense_b ; sparse_b]            (R = F+1 rows, D columns, R <= 32, D == 128)
 //   out_b = [dense_b , strict-upper-triangle(X_b X_b^T)]         (reference models/dlrm.py:210-222)
 //
-// The per-sample 27x27 products are far too small for a 128-row MMA, so FOUR samples are packed into
-// one 128 x 128 operand tile (32 rows per sample, unused rows zero) and ONE tcgen05.mma group
-// computes T T^T; only the four diagonal 32x32 blocks are read back (tcgen05.ld: TMEM lane == packed
-// row, so warp w owns sample w). The 4x redundant FLOPs are free (the kernel is HBM-bound) and the
-// operands never leave shared memory.
+// The per-sample 27x27 products are far too small for a 64-row MMA, so FOUR samples are packed into
+// one 128 x 128 operand tile (32 rows per sample, unused rows zero) in shared memory (SWIZZLE_128B).
+// The CTA is one warpgroup; each 64-row half (two samples) is multiplied with itself by wgmma
+// (m64n64k16, fp32 accumulators in registers) and only the two diagonal 32x32 blocks are kept.
+// The 2x redundant FLOPs are free (the kernel is HBM-bound) and the operands never leave shared memory.
 //
 // Backward: dX_b = S_b X_b with S_b the symmetric 27x27 matrix rebuilt from the triangle of the
 // incoming gradient. Tile math: D[128 x 128] = blockdiag(S)[128 x 128] . T[128 x 128] where the SAME
 // shared-memory image of T (row-major, SWIZZLE_128B) is consumed as an MN-major B operand — no transpose.
 //
-// CTAs are small (128 threads, ~38 KB smem, 128 TMEM columns) so 4 fit per SM and hide the global
-// load latency of each other; each CTA loops over groups of 4 samples.
+// CTAs are small (128 threads, ~38 KB smem) so several fit per SM and hide the global load latency of
+// each other; each CTA loops over groups of 4 samples.
 #include <cstdlib>
 
-#include "tcgen05.cuh"
+#include "wgmma.cuh"
 
 using namespace trb;
 
@@ -82,206 +82,6 @@ __device__ __forceinline__ void load_tile(const InterParams& p, uint8_t* tile, i
   }
 }
 
-__global__ void __launch_bounds__(128, 4) interaction_fwd_kernel(const InterParams p) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t) 1023);
-  uint8_t* tile = smem;                                            // 2 x 16 KB
-  __nv_bfloat16* stage = reinterpret_cast<__nv_bfloat16*>(smem + 2 * kTileBytes);  // [4][ld_out] output staging
-  uint64_t* bar = reinterpret_cast<uint64_t*>(smem + 2 * kTileBytes + kSamples * p.ld_out * 2);
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bar + 1);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int R = p.F + 1;
-
-  // zero the operand tile once: padding rows (i >= R) are never written again
-  for (int i = tid; i < 2 * kTileBytes / 16; i += 128) reinterpret_cast<uint4*>(tile)[i] = make_uint4(0, 0, 0, 0);
-  if (tid == 0) {
-    mbar_init(bar, 1);
-    fence_barrier_init();
-  }
-  if (warp == 0) tmem_alloc(tmem_ptr, 128);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_d = *tmem_ptr;
-  constexpr uint32_t idesc = make_idesc_major(128, 128, 0, 0);
-  uint32_t phase = 0;
-  const int groups = (p.B + kSamples - 1) / kSamples;
-  for (int g = blockIdx.x; g < groups; g += gridDim.x) {
-    const int b0 = g * kSamples;
-    load_tile(p, tile, b0, tid);
-    fence_proxy_async();  // generic-proxy smem writes -> visible to the tensor-core (async) proxy
-    __syncthreads();
-    if (warp == 0) {
-      if (elect_one()) {
-        const uint32_t a0 = smem_u32(tile);
-#pragma unroll
-        for (int kb = 0; kb < 2; ++kb) {
-          const uint64_t desc = make_kmajor_desc(a0 + kb * kTileBytes);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) umma_bf16(tmem_d, desc + (uint64_t) (2 * k), desc + (uint64_t) (2 * k), idesc, (kb | k) != 0);
-        }
-        umma_commit(bar);
-      }
-      __syncwarp();
-    }
-    mbar_wait(bar, phase);
-    phase ^= 1;
-    tc_fence_after();
-    // warp w <-> sample b0+w ; lane i <-> row i ; columns [32w, 32w+32) hold Z_w[i][0..31]
-    uint32_t z[32];
-    tmem_ld_32x32(tmem_d + ((uint32_t) (warp * 32) << 16) + (uint32_t) (warp * 32), z);
-    __nv_bfloat16* srow = stage + warp * p.ld_out;
-    if (lane < R) {
-      const int base = kD + tri_offset(lane, R);
-#pragma unroll
-      for (int j = 0; j < 32; ++j)
-        if (j > lane && j < R) srow[base + (j - lane - 1)] = __float2bfloat16(__uint_as_float(z[j]));
-    }
-    // dense passthrough + zero padding of the row tail
-    for (int c = lane; c < kD / 8; c += 32) {
-      const int r = warp * kRowsPerSample;
-      reinterpret_cast<uint4*>(srow)[c] = *reinterpret_cast<const uint4*>(tile + (c >> 3) * kTileBytes + sw128_offset(r, (c & 7) * 8));
-    }
-    for (int c = p.out_cols + lane; c < p.ld_out; c += 32) srow[c] = __float2bfloat16(0.f);
-    tc_fence_before();
-    __syncthreads();  // staging complete; TMEM + operand tile free for the next group
-    const int vec_per_row = (int) (p.ld_out >> 3);
-    for (int v = tid; v < kSamples * vec_per_row; v += 128) {
-      const int s = v / vec_per_row, c = v - s * vec_per_row;
-      if (b0 + s < p.B)
-        reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.out) + (int64_t) (b0 + s) * p.ld_out)[c] =
-            reinterpret_cast<const uint4*>(stage + s * p.ld_out)[c];
-    }
-    __syncthreads();
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem_d, 128);
-}
-
-__global__ void __launch_bounds__(128, 3) interaction_bwd_kernel(const InterParams p) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t) 1023);
-  uint8_t* tileT = smem;                     // packed X (2 K-blocks), used as MN-major B operand
-  uint8_t* tileS = smem + 2 * kTileBytes;    // block-diagonal S (2 K-blocks), K-major A operand
-  __nv_bfloat16* gstage = reinterpret_cast<__nv_bfloat16*>(smem + 4 * kTileBytes);  // [4][ld_out] incoming gradient rows
-  uint64_t* bar = reinterpret_cast<uint64_t*>(smem + 4 * kTileBytes + kSamples * p.ld_out * 2);
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bar + 1);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int R = p.F + 1;
-
-  for (int i = tid; i < 4 * kTileBytes / 16; i += 128) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
-  if (tid == 0) {
-    mbar_init(bar, 1);
-    fence_barrier_init();
-  }
-  if (warp == 0) tmem_alloc(tmem_ptr, 128);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_d = *tmem_ptr;
-  // A: K-major (block-diagonal S), B: MN-major (packed X, [k = packed row][n = dim])
-  constexpr uint32_t idesc = make_idesc_major(128, 128, 0, 1);
-  uint32_t phase = 0;
-  const int groups = (p.B + kSamples - 1) / kSamples;
-  for (int g = blockIdx.x; g < groups; g += gridDim.x) {
-    const int b0 = g * kSamples;
-    load_tile(p, tileT, b0, tid);
-    // stage the 4 incoming gradient rows with coalesced 16 B loads
-    {
-      const int vec_per_row = (int) (p.ld_out >> 3);
-      for (int v = tid; v < kSamples * vec_per_row; v += 128) {
-        const int sidx = v / vec_per_row, c = v - sidx * vec_per_row;
-        uint4 val = make_uint4(0, 0, 0, 0);
-        if (b0 + sidx < p.B) val = reinterpret_cast<const uint4*>(reinterpret_cast<const __nv_bfloat16*>(p.gout) + (int64_t) (b0 + sidx) * p.ld_out)[c];
-        reinterpret_cast<uint4*>(gstage + sidx * p.ld_out)[c] = val;
-      }
-    }
-    __syncthreads();
-    // S rows: thread (warp = sample, lane = i) writes S[i][j] for all j (symmetric, zero diagonal)
-    {
-      const int b = b0 + warp;
-      const int r = warp * kRowsPerSample + lane;
-      const __nv_bfloat16* grow = gstage + warp * p.ld_out + kD;
-      if (lane < R) {
-        for (int j = 0; j < R; ++j) {
-          __nv_bfloat16 v = __float2bfloat16(0.f);
-          if (b < p.B && j != lane) {
-            const int lo = min(lane, j), hi = max(lane, j);
-            v = grow[tri_offset(lo, R) + (hi - lo - 1)];
-          }
-          const int k = warp * kRowsPerSample + j;
-          *reinterpret_cast<__nv_bfloat16*>(tileS + (k >> 6) * kTileBytes + sw128_offset(r, k & 63)) = v;
-        }
-      }
-    }
-    fence_proxy_async();
-    __syncthreads();
-    if (warp == 0) {
-      if (elect_one()) {
-        const uint32_t aS = smem_u32(tileS), aT = smem_u32(tileT);
-#pragma unroll
-        for (int kb = 0; kb < 2; ++kb) {
-          const uint64_t adesc = make_kmajor_desc(aS + kb * kTileBytes);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            // B: K index = packed row (kb*64 + k*16 ...): 16 rows x 128 B = 2048 B per UMMA_K step inside
-            // the [128 rows x 128 B] image; the two 64-column halves (MN atoms) are kTileBytes apart.
-            const uint64_t bdesc = make_mnmajor_desc(aT + (kb * 64 + k * 16) * 128, kTileBytes, 1024);
-            umma_bf16(tmem_d, adesc + (uint64_t) (2 * k), bdesc, idesc, (kb | k) != 0);
-          }
-        }
-        umma_commit(bar);
-      }
-      __syncwarp();
-    }
-    mbar_wait(bar, phase);
-    phase ^= 1;
-    tc_fence_after();
-    const int b = b0 + warp;
-    const bool ok = b < p.B && lane < R;
-#pragma unroll 1
-    for (int c = 0; c < 4; ++c) {
-      uint32_t z[32];
-      tmem_ld_32x32(tmem_d + ((uint32_t) (warp * 32) << 16) + (uint32_t) (c * 32), z);
-      if (!ok) continue;
-      float v[32];
-#pragma unroll
-      for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(z[j]);
-      if (lane == 0) {
-        // dense row: add the pass-through gradient of out[:, :D]
-        const __nv_bfloat16* gd = gstage + warp * p.ld_out + c * 32;
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] += __bfloat162float(gd[j]);
-        __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(p.g_dense) + (int64_t) b * p.ld_gdense + c * 32;
-#pragma unroll
-        for (int j = 0; j < 32; j += 2) *reinterpret_cast<__nv_bfloat162*>(dst + j) = __floats2bfloat162_rn(v[j], v[j + 1]);
-      } else if (p.gsparse_f32) {
-        float* dst = reinterpret_cast<float*>(p.g_sparse) + (int64_t) b * p.ld_gsparse + (lane - 1) * kD + c * 32;
-#pragma unroll
-        for (int j = 0; j < 32; j += 4) *reinterpret_cast<float4*>(dst + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-      } else {
-        __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(p.g_sparse) + (int64_t) b * p.ld_gsparse + (lane - 1) * kD + c * 32;
-#pragma unroll
-        for (int j = 0; j < 32; j += 2) *reinterpret_cast<__nv_bfloat162*>(dst + j) = __floats2bfloat162_rn(v[j], v[j + 1]);
-      }
-    }
-    tc_fence_before();
-    __syncthreads();
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem_d, 128);
-}
-
-
-// ================================================================================================================
-// Pipelined bf16 kernels (the production path): operand tiles arrive through cp.async (16 B LDGSTS, every thread has
-// all of its loads in flight at once) into a DOUBLE-BUFFERED smem image, so the global->smem traffic of group g+1
-// overlaps the MMA + epilogue of group g; results leave through a swizzled smem staging area with fully coalesced
-// 16 B stores. The first-generation kernels above (synchronous loads, per-thread 4 B stores) ran at 17-27 % of the HBM
-// roofline (profiles/step_breakdown_1gpu_r1.md) and remain as the fp32-I/O fallback.
-// ================================================================================================================
 __device__ __forceinline__ void cp_async16(uint32_t smem_addr, const void* g, bool valid) {
   const int sz = valid ? 16 : 0;  // src-size 0 -> zero fill
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_addr), "l"(g), "r"(sz) : "memory");
@@ -291,7 +91,7 @@ __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wai
 
 // issue (do not wait for) the loads of the packed tile of samples [b0, b0+4): bf16 dense + bf16 sparse.
 // Thread t always moves column chunk (t & 15) of rows (t >> 4) + 8k, so the swizzle term and all strides are per-thread
-// constants (the first version recomputed them per chunk and was instruction-bound, profiles/ncu_interaction_bwd_pipe_kernel_r1.md).
+// constants (recomputing them per chunk made the kernel instruction-bound).
 // EXTRA: also load gout[b][0:128] (the pass-through gradient of the dense row) as packed row R, so the backward MMA adds it
 // in fp32 through S[0][R] = 1 instead of a lane-0 epilogue special case.
 template <bool EXTRA>
@@ -333,24 +133,198 @@ __device__ __forceinline__ void issue_gout_loads(const InterParams& p, __nv_bflo
   }
 }
 
+// ---- tensor-core pieces shared by the kernels (all 128 threads = one warpgroup; warp w, lane l) ----------------------
+// Forward: Z = T T^T is only needed on the four diagonal 32 x 32 blocks. wgmma M-half h (packed rows [64h, 64h + 64) =
+// samples 2h, 2h + 1) is multiplied with the same 64 rows only (N = 64): 2 x (m64n64k16 x 8) instead of a 128 x 128 product.
+__device__ __forceinline__ void fwd_mma_issue(uint32_t tile_addr, float (&z)[2][32]) {
+  wgmma_fence();
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int kb = 0; kb < 2; ++kb)
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const uint64_t desc = make_kmajor_desc(tile_addr + kb * kTileBytes + h * 8192 + k * 32);
+        wgmma_m64n64k16<0, 0>(z[h], desc, desc, (kb | k) != 0);
+      }
+  wgmma_commit();
+}
+
+__device__ __forceinline__ void mma_wait(float (&z)[2][32]) {
+  wgmma_wait<0>();
+  wgmma_fence_regs(z[0]);
+  wgmma_fence_regs(z[1]);
+}
+
+// strict upper triangle of the diagonal blocks -> the staged output rows (stage[s][kD + tri(i) + (j - i - 1)])
+__device__ __forceinline__ void fwd_scatter(const float (&z)[2][32], __nv_bfloat16* stage, int64_t ld_out, int R, int warp, int lane) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+          const int row = 16 * warp + (lane >> 2) + 8 * hh, col = 8 * j + 2 * (lane & 3) + c;  // inside M-half h
+          const int i = row & 31, jj = col & 31;
+          if ((row >> 5) == (col >> 5) && i < jj && jj < R)
+            stage[(2 * h + (row >> 5)) * ld_out + kD + tri_offset(i, R) + (jj - i - 1)] = __float2bfloat16(z[h][4 * j + 2 * hh + c]);
+        }
+}
+
+// Backward: D = blockdiag(S) . T. M-half h of blockdiag(S) is zero outside K-block h, so each half is 4 x m64n128k16 with
+// A = S (K-major) and B = T consumed MN-major ([k = packed row][n = dim]; the two 64-column halves are kTileBytes apart).
+// The halves run one after the other (64 accumulator registers instead of 128). Half h reads only rows [64h, 64h + 64) of K-block h
+// of S, so the output of half 0 may already overwrite K-block 0 while half 1 runs.
+__device__ __forceinline__ void bwd_mma_half(uint32_t aS, uint32_t aT, int h, float (&d)[64]) {
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const uint64_t adesc = make_kmajor_desc(aS + h * kTileBytes + h * 8192 + k * 32);
+    const uint64_t bdesc = make_smem_desc(aT + (h * 64 + k * 16) * 128, kTileBytes, 1024);
+    wgmma_m64n128k16<0, 1>(d, adesc, bdesc, k != 0);
+  }
+  wgmma_commit();
+  wgmma_wait<0>();
+  wgmma_fence_regs(d);
+}
+
+__global__ void __launch_bounds__(128, 4) interaction_fwd_kernel(const InterParams p) {
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t) 1023);
+  uint8_t* tile = smem;                                            // 2 x 16 KB
+  __nv_bfloat16* stage = reinterpret_cast<__nv_bfloat16*>(smem + 2 * kTileBytes);  // [4][ld_out] output staging
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int R = p.F + 1;
+
+  // zero the operand tile once: padding rows (i >= R) are never written again
+  for (int i = tid; i < 2 * kTileBytes / 16; i += 128) reinterpret_cast<uint4*>(tile)[i] = make_uint4(0, 0, 0, 0);
+  __syncthreads();
+  const int groups = (p.B + kSamples - 1) / kSamples;
+  for (int g = blockIdx.x; g < groups; g += gridDim.x) {
+    const int b0 = g * kSamples;
+    load_tile(p, tile, b0, tid);
+    fence_proxy_async();  // generic-proxy smem writes -> visible to the tensor-core (async) proxy
+    __syncthreads();
+    float z[2][32];
+    fwd_mma_issue(smem_u32(tile), z);
+    mma_wait(z);
+    fwd_scatter(z, stage, p.ld_out, R, warp, lane);
+    // dense passthrough + zero padding of the row tail (warp w <-> sample b0 + w)
+    __nv_bfloat16* srow = stage + warp * p.ld_out;
+    for (int c = lane; c < kD / 8; c += 32) {
+      const int r = warp * kRowsPerSample;
+      reinterpret_cast<uint4*>(srow)[c] = *reinterpret_cast<const uint4*>(tile + (c >> 3) * kTileBytes + sw128_offset(r, (c & 7) * 8));
+    }
+    for (int c = p.out_cols + lane; c < p.ld_out; c += 32) srow[c] = __float2bfloat16(0.f);
+    __syncthreads();  // staging complete; operand tile free for the next group
+    const int vec_per_row = (int) (p.ld_out >> 3);
+    for (int v = tid; v < kSamples * vec_per_row; v += 128) {
+      const int s = v / vec_per_row, c = v - s * vec_per_row;
+      if (b0 + s < p.B)
+        reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.out) + (int64_t) (b0 + s) * p.ld_out)[c] =
+            reinterpret_cast<const uint4*>(stage + s * p.ld_out)[c];
+    }
+    __syncthreads();
+  }
+}
+
+__global__ void __launch_bounds__(128, 3) interaction_bwd_kernel(const InterParams p) {
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t) 1023);
+  uint8_t* tileT = smem;                     // packed X (2 K-blocks), used as MN-major B operand
+  uint8_t* tileS = smem + 2 * kTileBytes;    // block-diagonal S (2 K-blocks), K-major A operand
+  __nv_bfloat16* gstage = reinterpret_cast<__nv_bfloat16*>(smem + 4 * kTileBytes);  // [4][ld_out] incoming gradient rows
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int R = p.F + 1;
+
+  for (int i = tid; i < 4 * kTileBytes / 16; i += 128) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
+  __syncthreads();
+  const int groups = (p.B + kSamples - 1) / kSamples;
+  for (int g = blockIdx.x; g < groups; g += gridDim.x) {
+    const int b0 = g * kSamples;
+    load_tile(p, tileT, b0, tid);
+    // stage the 4 incoming gradient rows with coalesced 16 B loads
+    {
+      const int vec_per_row = (int) (p.ld_out >> 3);
+      for (int v = tid; v < kSamples * vec_per_row; v += 128) {
+        const int sidx = v / vec_per_row, c = v - sidx * vec_per_row;
+        uint4 val = make_uint4(0, 0, 0, 0);
+        if (b0 + sidx < p.B) val = reinterpret_cast<const uint4*>(reinterpret_cast<const __nv_bfloat16*>(p.gout) + (int64_t) (b0 + sidx) * p.ld_out)[c];
+        reinterpret_cast<uint4*>(gstage + sidx * p.ld_out)[c] = val;
+      }
+    }
+    __syncthreads();
+    // S rows: thread (warp = sample, lane = i) writes S[i][j] for all j (symmetric, zero diagonal)
+    {
+      const int b = b0 + warp;
+      const int r = warp * kRowsPerSample + lane;
+      const __nv_bfloat16* grow = gstage + warp * p.ld_out + kD;
+      if (lane < R) {
+        for (int j = 0; j < R; ++j) {
+          __nv_bfloat16 v = __float2bfloat16(0.f);
+          if (b < p.B && j != lane) {
+            const int lo = min(lane, j), hi = max(lane, j);
+            v = grow[tri_offset(lo, R) + (hi - lo - 1)];
+          }
+          const int k = warp * kRowsPerSample + j;
+          *reinterpret_cast<__nv_bfloat16*>(tileS + (k >> 6) * kTileBytes + sw128_offset(r, k & 63)) = v;
+        }
+      }
+    }
+    fence_proxy_async();
+    __syncthreads();
+    const int q = lane & 3;
+#pragma unroll 1
+    for (int h = 0; h < 2; ++h) {
+      float d[64];
+      bwd_mma_half(smem_u32(tileS), smem_u32(tileT), h, d);
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int r = 64 * h + 16 * warp + (lane >> 2) + 8 * hh;
+        const int s = r >> 5, i = r & 31, b = b0 + s;
+        if (b >= p.B || i >= R) continue;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const int col = 8 * j + 2 * q;
+          float v0 = d[4 * j + 2 * hh], v1 = d[4 * j + 2 * hh + 1];
+          if (i == 0) {
+            // dense row: add the pass-through gradient of out[:, :D]
+            const __nv_bfloat162 gd = *reinterpret_cast<const __nv_bfloat162*>(gstage + s * p.ld_out + col);
+            v0 += __bfloat162float(gd.x);
+            v1 += __bfloat162float(gd.y);
+            *reinterpret_cast<__nv_bfloat162*>(reinterpret_cast<__nv_bfloat16*>(p.g_dense) + (int64_t) b * p.ld_gdense + col) = __floats2bfloat162_rn(v0, v1);
+          } else if (p.gsparse_f32) {
+            *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.g_sparse) + (int64_t) b * p.ld_gsparse + (i - 1) * kD + col) = make_float2(v0, v1);
+          } else {
+            *reinterpret_cast<__nv_bfloat162*>(reinterpret_cast<__nv_bfloat16*>(p.g_sparse) + (int64_t) b * p.ld_gsparse + (i - 1) * kD + col) =
+                __floats2bfloat162_rn(v0, v1);
+          }
+        }
+      }
+    }
+    __syncthreads();
+  }
+}
+
+
+// ================================================================================================================
+// Pipelined bf16 kernels (the production path): operand tiles arrive through cp.async (16 B LDGSTS, every thread has
+// all of its loads in flight at once) into a DOUBLE-BUFFERED smem image, so the global->smem traffic of group g+1
+// overlaps the MMA + epilogue of group g; results leave through a swizzled smem staging area with fully coalesced
+// 16 B stores. The kernels above (synchronous loads, per-thread 4 B stores) remain as the fp32-I/O fallback.
+// ================================================================================================================
+
 __global__ void __launch_bounds__(128, 3) interaction_fwd_pipe_kernel(const InterParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t) 1023);
   uint8_t* tiles = smem;                                                               // 2 buffers x (2 x 16 KB)
   __nv_bfloat16* stage = reinterpret_cast<__nv_bfloat16*>(smem + 4 * kTileBytes);      // [4][ld_out]
-  uint64_t* bar = reinterpret_cast<uint64_t*>(smem + 4 * kTileBytes + kSamples * p.ld_out * 2);
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bar + 1);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int R = p.F + 1;
   for (int i = tid; i < 4 * kTileBytes / 16; i += 128) reinterpret_cast<uint4*>(tiles)[i] = make_uint4(0, 0, 0, 0);
-  if (tid == 0) { mbar_init(bar, 1); fence_barrier_init(); }
-  if (warp == 0) tmem_alloc(tmem_ptr, 128);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_d = *tmem_ptr;
-  constexpr uint32_t idesc = make_idesc_major(128, 128, 0, 0);
-  uint32_t phase = 0;
   const int groups = (p.B + kSamples - 1) / kSamples;
   int cur = 0;
   if ((int) blockIdx.x < groups) issue_tile_loads<false>(p, tiles, blockIdx.x * kSamples, tid);
@@ -363,19 +337,8 @@ __global__ void __launch_bounds__(128, 3) interaction_fwd_pipe_kernel(const Inte
     __syncthreads();  // tile[cur] landed; everyone is done with tile[cur^1] and with `stage`
     if (g + (int) gridDim.x < groups) issue_tile_loads<false>(p, tiles + (cur ^ 1) * 2 * kTileBytes, (g + gridDim.x) * kSamples, tid);
     cp_async_commit();
-    if (warp == 0) {
-      if (elect_one()) {
-        const uint32_t a0 = smem_u32(tile);
-#pragma unroll
-        for (int kb = 0; kb < 2; ++kb) {
-          const uint64_t desc = make_kmajor_desc(a0 + kb * kTileBytes);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) umma_bf16(tmem_d, desc + (uint64_t) (2 * k), desc + (uint64_t) (2 * k), idesc, (kb | k) != 0);
-        }
-        umma_commit(bar);
-      }
-      __syncwarp();
-    }
+    float z[2][32];
+    fwd_mma_issue(smem_u32(tile), z);
     // dense passthrough + zero tail while the MMA runs
     __nv_bfloat16* srow = stage + warp * p.ld_out;
     for (int c = lane; c < kD / 8; c += 32) {
@@ -383,18 +346,8 @@ __global__ void __launch_bounds__(128, 3) interaction_fwd_pipe_kernel(const Inte
       reinterpret_cast<uint4*>(srow)[c] = *reinterpret_cast<const uint4*>(tile + (c >> 3) * kTileBytes + sw128_offset(r, (c & 7) * 8));
     }
     for (int c = p.out_cols + lane; c < p.ld_out; c += 32) srow[c] = __float2bfloat16(0.f);
-    mbar_wait(bar, phase);
-    phase ^= 1;
-    tc_fence_after();
-    uint32_t z[32];
-    tmem_ld_32x32(tmem_d + ((uint32_t) (warp * 32) << 16) + (uint32_t) (warp * 32), z);
-    if (lane < R) {
-      const int base = kD + tri_offset(lane, R);
-#pragma unroll
-      for (int j = 0; j < 32; ++j)
-        if (j > lane && j < R) srow[base + (j - lane - 1)] = __float2bfloat16(__uint_as_float(z[j]));
-    }
-    tc_fence_before();
+    mma_wait(z);
+    fwd_scatter(z, stage, p.ld_out, R, warp, lane);
     __syncthreads();
     const int vec_per_row = (int) (p.ld_out >> 3);
 #pragma unroll
@@ -406,9 +359,6 @@ __global__ void __launch_bounds__(128, 3) interaction_fwd_pipe_kernel(const Inte
     }
   }
   cp_async_wait_all();
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem_d, 128);
 }
 
 template <bool EXTRA>
@@ -418,19 +368,10 @@ __global__ void __launch_bounds__(128, 2) interaction_bwd_pipe_kernel(const Inte
   uint8_t* tiles = smem;                       // T: 2 buffers x 32 KB (MN-major B operand)
   uint8_t* tileS = smem + 4 * kTileBytes;      // S (K-major A operand, 32 KB); re-used as the output staging area after the MMA
   __nv_bfloat16* gst = reinterpret_cast<__nv_bfloat16*>(smem + 6 * kTileBytes);  // 2 x [4][ld_out]
-  uint64_t* bar = reinterpret_cast<uint64_t*>(smem + 6 * kTileBytes + 2 * kSamples * p.ld_out * 2);
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bar + 1);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int R = p.F + 1;
   for (int i = tid; i < 4 * kTileBytes / 16; i += 128) reinterpret_cast<uint4*>(tiles)[i] = make_uint4(0, 0, 0, 0);
-  if (tid == 0) { mbar_init(bar, 1); fence_barrier_init(); }
-  if (warp == 0) tmem_alloc(tmem_ptr, 128);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_d = *tmem_ptr;
-  constexpr uint32_t idesc = make_idesc_major(128, 128, 0, 1);
-  uint32_t phase = 0;
   const int groups = (p.B + kSamples - 1) / kSamples;
   const int gsz = kSamples * (int) p.ld_out;
   int cur = 0;
@@ -493,51 +434,29 @@ __global__ void __launch_bounds__(128, 2) interaction_bwd_pipe_kernel(const Inte
     }
     fence_proxy_async();
     __syncthreads();
-    if (warp == 0) {
-      if (elect_one()) {
-        const uint32_t aS = smem_u32(tileS), aT = smem_u32(tileT);
-#pragma unroll
-        for (int kb = 0; kb < 2; ++kb) {
-          const uint64_t adesc = make_kmajor_desc(aS + kb * kTileBytes);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const uint64_t bdesc = make_mnmajor_desc(aT + (kb * 64 + k * 16) * 128, kTileBytes, 1024);
-            umma_bf16(tmem_d, adesc + (uint64_t) (2 * k), bdesc, idesc, (kb | k) != 0);
-          }
-        }
-        umma_commit(bar);
-      }
-      __syncwarp();
-    }
-    mbar_wait(bar, phase);
-    phase ^= 1;
-    tc_fence_after();
-    // ---- epilogue: TMEM -> bf16 -> swizzled staging ([128 rows][16 chunks of 16 B], chunk ^= row & 15) -----------------
+    // ---- per half: MMA, then registers -> bf16 -> swizzled staging ([128 rows][16 chunks of 16 B], chunk ^= row & 15). The
+    //      staging rows of half h are K-block h of S, which only half h reads: its wgmma has retired when the stores start.
     uint8_t* ostage = tileS;
+    const int q = lane & 3;
 #pragma unroll 1
-    for (int c = 0; c < 4; ++c) {
-      uint32_t z[32];
-      tmem_ld_32x32(tmem_d + ((uint32_t) (warp * 32) << 16) + (uint32_t) (c * 32), z);
-      float v[32];
+    for (int h = 0; h < 2; ++h) {
+      float d[64];
+      bwd_mma_half(smem_u32(tileS), smem_u32(tileT), h, d);
 #pragma unroll
-      for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(z[j]);
-      if (!EXTRA && lane == 0) {  // R == 32: no spare packed row, add the pass-through gradient of out[:, :D] here
-        const __nv_bfloat16* gd = gstage + warp * p.ld_out + c * 32;
+      for (int hh = 0; hh < 2; ++hh) {
+        const int rr = 64 * h + 16 * warp + (lane >> 2) + 8 * hh;
 #pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] += __bfloat162float(gd[j]);
-      }
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        uint4 o;
-        __nv_bfloat162 h0 = __floats2bfloat162_rn(v[8 * q], v[8 * q + 1]), h1 = __floats2bfloat162_rn(v[8 * q + 2], v[8 * q + 3]);
-        __nv_bfloat162 h2 = __floats2bfloat162_rn(v[8 * q + 4], v[8 * q + 5]), h3 = __floats2bfloat162_rn(v[8 * q + 6], v[8 * q + 7]);
-        o.x = *reinterpret_cast<uint32_t*>(&h0); o.y = *reinterpret_cast<uint32_t*>(&h1);
-        o.z = *reinterpret_cast<uint32_t*>(&h2); o.w = *reinterpret_cast<uint32_t*>(&h3);
-        const int chunk = c * 4 + q;
-        *reinterpret_cast<uint4*>(ostage + r * 256 + (((chunk ^ lane) & 15) << 4)) = o;
+        for (int j = 0; j < 16; ++j) {
+          float v0 = d[4 * j + 2 * hh], v1 = d[4 * j + 2 * hh + 1];
+          if (!EXTRA && (rr & 31) == 0) {  // R == 32: no spare packed row, add the pass-through gradient of out[:, :D] here
+            const __nv_bfloat162 gd = *reinterpret_cast<const __nv_bfloat162*>(gstage + (rr >> 5) * p.ld_out + 8 * j + 2 * q);
+            v0 += __bfloat162float(gd.x);
+            v1 += __bfloat162float(gd.y);
+          }
+          *reinterpret_cast<__nv_bfloat162*>(ostage + rr * 256 + (((j ^ rr) & 15) << 4) + 4 * q) = __floats2bfloat162_rn(v0, v1);
+        }
       }
     }
-    tc_fence_before();
     __syncthreads();
     // ---- coalesced copy-out: 16 consecutive threads write one 256 B gradient row; thread t owns chunk (t & 15) of rows (t >> 4) + 8k
     {
@@ -560,9 +479,6 @@ __global__ void __launch_bounds__(128, 2) interaction_bwd_pipe_kernel(const Inte
     }
   }
   cp_async_wait_all();
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem_d, 128);
 }
 
 int g_sms = 0;

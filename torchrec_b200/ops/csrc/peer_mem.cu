@@ -3,7 +3,7 @@
 // collectives need (staging reduce, cast-copy into a symmetric buffer).
 //
 // This replaces NCCL on the embedding hot paths: kernels receive the peers' buffer addresses and
-// load/store them directly over NVSwitch (B300_MICROARCH.md "NVLink": peer LDG.128 ~775 GB/s).
+// load/store them directly over NVSwitch.
 // NCCL stays the control plane (handle exchange, DDP all-reduce, multi-node fallback).
 #include "common.cuh"
 #include <cstdlib>
@@ -226,14 +226,14 @@ TRB_API int trb_cast_copy(const void* src, int s_dtype, void* dst, int d_dtype, 
 // gradient [B_local, total_cols] to the ranks that own the corresponding table shards, into THEIR gradient inbox
 // [W * B_local, pitch] at rows [src_rank * B_local, ...). Chunks of 4 elements are described by a small device table
 // (dst rank, src col, dst col). Posted remote writes pipeline far deeper than the remote row *reads* of a pull design
-// (peer load latency ~1.8k cycles, B300_MICROARCH.md), and the fused backward afterwards only touches local HBM.
+// (a peer load is a full NVLink round trip), and the fused backward afterwards only touches local HBM.
 // Parity: the backward all_to_all_single of the pooled output dist (reference comm_ops.py:1581-1646).
 // ---------------------------------------------------------------------------------------------------------------
 // VEC = elements per chunk (4 or 8). 8-element chunks move 16 B per thread for bf16 gradients.
 //
 // PERSISTENT, narrow launch: the kernel is NVLink-bound (posted peer stores), it needs bytes in flight, not thread slots. The
 // first version launched one thread per chunk (53 k blocks for a DLRM batch): those blocks filled every thread slot of every SM for
-// the whole transfer and starved the weight-gradient GEMMs that are meant to run beside it (timeline: profiles/timeline_n2_r2.md).
+// the whole transfer and starved the weight-gradient GEMMs that are meant to run beside it.
 // Now ~2 CTAs per SM walk the chunks with a grid stride, UNR independent 16 B loads in flight per thread before the stores.
 template <typename S, typename D, int VEC, int UNR>
 __global__ void __launch_bounds__(256)
@@ -298,7 +298,7 @@ TRB_API int trb_grad_push(const void* src, int s_dtype, int64_t src_stride, cons
   const int threads = 256;
   constexpr int UNR = 4;
   static const int ctas_per_sm = getenv("TRB_PUSH_CTAS_PER_SM") ? atoi(getenv("TRB_PUSH_CTAS_PER_SM")) : 2;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   int64_t want = (n + (int64_t) threads * UNR - 1) / ((int64_t) threads * UNR);

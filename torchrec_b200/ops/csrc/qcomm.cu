@@ -1,4 +1,4 @@
-// Quantized-communication codecs (sm_100a): what travels on the wire of the pooled / sequence embedding collectives when a
+// Quantized-communication codecs (sm_90a): what travels on the wire of the pooled / sequence embedding collectives when a
 // `QCommsConfig` asks for less than fp32 (reference torchrec/distributed/fbgemm_qcomm_codec.py:31-254, fbgemm quantize_comm):
 //
 //   FP8 row-wise   per row of `row_dim` elements: e4m3 payload + one fp32 scale (amax / 448), layout [rows][row_dim + 4 bytes]

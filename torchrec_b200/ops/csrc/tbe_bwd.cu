@@ -1,4 +1,4 @@
-// Table-batched embedding backward fused with the sparse optimizer (sm_100a).
+// Table-batched embedding backward fused with the sparse optimizer (sm_90a).
 //
 // Exact (deterministic, duplicate-safe) semantics like the reference's EXACT_* TBE optimizers
 // (torchrec/distributed/embedding_types.py:57-72; fused backward reached through autograd at
@@ -367,8 +367,7 @@ __device__ __forceinline__ void load_grad_row(const TbeBwdParams& p, int bag, fl
 // chunk_done so the generic walk (tbe_bwd_chunk_kernel, lighter on registers, higher occupancy) skips them. Per-lane geometry
 // is computed ONCE in parallel (the generic walk re-derives it per row with integer divisions on every lane) and rows are
 // processed U at a time with all of their gradient / weight / state loads in flight together. The generic path alone was
-// instruction- and latency-bound: 182 warp instructions per id, one row in flight per warp
-// (profiles/ncu_tbe_bwd_chunk_kernel_r1.md).
+// instruction- and latency-bound: one row in flight per warp.
 template <typename W, typename G, int MAXV>
 __global__ void __launch_bounds__(256) tbe_bwd_unique_kernel(const TbeBwdParams p) {
   typedef uint64_t K;
@@ -469,8 +468,7 @@ __global__ void __launch_bounds__(256) tbe_bwd_unique_kernel(const TbeBwdParams 
 
 // ---- multi-row walk ---------------------------------------------------------------------------------------------------
 // The generic walk below handles one run of equal keys at a time: gradient rows -> weight row -> row state -> store is ONE dependent
-// chain per warp, and every lane re-derives the row geometry (two integer divisions) for every gradient row: 182 warp instructions
-// per id at 48 % issue utilisation, 2 TB/s (profiles/ncu_tbe_bwd_chunk_kernel_r1.md). For SGD / row-wise Adagrad without clipping
+// chain per warp, and every lane re-derives the row geometry (two integer divisions) for every gradient row. For SGD / row-wise Adagrad without clipping
 // or weight decay this kernel walks the same 32 sorted keys U entries at a time instead:
 //   * geometry (gradient offset, weight offset, scale, source rank) is computed once, one entry per lane, and broadcast by shuffles;
 //   * the U gradient rows AND the weight rows / row states of the runs that end inside the group are all requested before any of
@@ -591,8 +589,7 @@ __global__ void __launch_bounds__(256, MINB) tbe_bwd_walk_kernel(const TbeBwdPar
     }
     // Group of U DISTINCT rows that all live inside the chunk (the common case for large tables): the U updates are independent, so
     // their square-sum reductions, square roots and divisions are interleaved instead of running as U dependent chains back to back
-    // (with one warp per scheduler-slot nothing else hides that latency: row-wise Adagrad was 436 us where SGD took 294 us for the
-    // same 1 M rows). Same arithmetic, same order per row as the sequential path below: bit-identical results.
+    // (with one warp per scheduler-slot nothing else hides that latency). Same arithmetic, same order per row as the sequential path below: bit-identical results.
     if constexpr (U > 1) {
       constexpr unsigned kAll = (1u << U) - 1u;
       const bool distinct = j + U <= cnt_v && ((ends >> j) & kAll) == kAll && (j == 0 || ((ends >> (j - 1)) & 1u)) &&
@@ -714,7 +711,7 @@ __global__ void __launch_bounds__(256) tbe_bwd_chunk_kernel(const TbeBwdParams p
   const bool is_start = (lane == 0) || (key != up);
   unsigned starts = __ballot_sync(0xffffffffu, lane < cnt && is_start);
   // The walk below is one dependent chain per run (gradient rows -> weight row -> optimizer state -> store): ~3 DRAM round
-  // trips per row with a single row in flight per warp made this kernel latency bound at 2 TB/s. Every lane therefore
+  // trips per row with a single row in flight per warp made this kernel latency bound. Every lane therefore
   // software-prefetches the lines of ITS key (weight row, gradient row, row state) into L2 a few runs before the walk reaches
   // it, so the chain hits L2 (~250 cycles) instead of HBM. kPrefetchAhead keys in flight per warp keeps the footprint small.
   constexpr int kPrefetchAhead = 6;
@@ -755,8 +752,8 @@ __global__ void __launch_bounds__(256) tbe_bwd_chunk_kernel(const TbeBwdParams p
     const int f = __shfl_sync(0xffffffffu, bag, a) / p.B;
     const bool head_open = (a == 0) && has_prev && (rk == prev_key);
     const bool tail_open = (bnd == cnt) && has_next && (rk == next_key);
-    // (loading the weight row / row state HERE, before the gradient gather, was tried: +7 registers, 278 -> 288 us. With the L2
-    // prefetch above the in-order loads of apply_row already hit L2.)
+    // (the weight row / row state are loaded after the gradient gather: with the L2 prefetch above the in-order loads of apply_row
+    // already hit L2, and loading them here costs registers.)
     float4 acc[MAXV];
 #pragma unroll
     for (int k = 0; k < MAXV; ++k) acc[k] = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -788,8 +785,8 @@ __global__ void __launch_bounds__(256) tbe_bwd_chunk_kernel(const TbeBwdParams p
 // A run of equal keys that crosses chunk boundaries left one partial row per chunk: slot 1 of its first chunk (flagged), slot 0
 // of every following chunk. One WARP per flagged chunk sums the pieces and applies the optimizer (short spans are the common
 // case: mid-size tables); spans longer than kLongSpan pieces (hot rows of tiny tables) are deferred to a worklist processed by
-// whole blocks in tbe_bwd_span_long_kernel. (The first version used one 256-thread block per chunk: 26 k mostly-empty blocks
-// cost 107 us; a later compact grid serialised neighbouring spans inside one block and cost 394 us.)
+// whole blocks in tbe_bwd_span_long_kernel. (One 256-thread block per chunk would launch mostly-empty blocks; a compact grid would
+// serialise neighbouring spans inside one block.)
 constexpr int kLongSpan = 24;
 
 template <int MAXV>
@@ -825,7 +822,7 @@ __device__ __forceinline__ void span_accumulate(const TbeBwdParams& p, int64_t c
 
 // Last chunk of the run of equal keys that leaves chunk c through its last entry. Called by whole warps: a 32-ary search (every lane
 // probes one point per step, 4 steps over 1 M keys) instead of a 20-step binary search of dependent loads - the search was most of
-// the latency of the span kernels (profiles/kernel_roofline_r2.md).
+// the latency of the span kernels.
 __device__ __forceinline__ int64_t span_last_chunk(const TbeBwdParams& p, int64_t c, uint64_t* rk_out) {
   const int lane = threadIdx.x & 31;
   const int64_t last = c * 32 + 31;
@@ -872,7 +869,7 @@ __global__ void __launch_bounds__(256) tbe_bwd_span_kernel(const TbeBwdParams p)
 }
 
 // kLongWarps warps per long span: at 8 GPUs the global batch makes the hot rows of the tiny tables 8x longer (a 3-row table: 87 k entries
-// per row = 2730 partial rows); with 8 warps per span this kernel was 81 us at the very end of the step (profiles/step_kernels_n8_r2.md).
+// per row = 2730 partial rows), and this kernel runs at the very end of the step.
 constexpr int kLongWarps = 32;
 
 template <typename W, int MAXV>
@@ -993,13 +990,14 @@ static int run_bwd(TbeBwdParams& p, char* ws, cudaStream_t stream) {
   const int64_t chunks = (p.n + 31) / 32;
   const int64_t blocks = (chunks + 7) / 8;
   // pass 1 (optional): chunks of distinct rows with a simple optimizer go through the high-MLP unique kernel
-  static const int fast_enabled = getenv("TRB_BWD_UNIQUE") ? atoi(getenv("TRB_BWD_UNIQUE")) : 0;  // measured slower than the generic walk on B200 so far: opt-in
+  static const int fast_enabled = getenv("TRB_BWD_UNIQUE") ? atoi(getenv("TRB_BWD_UNIQUE")) : 0;  // opt-in
   static const int walk_enabled = getenv("TRB_BWD_WALK") ? atoi(getenv("TRB_BWD_WALK")) : 1;
   const bool simple_opt = (p.opt == OPT_SGD || p.opt == OPT_ROWWISE_ADAGRAD) && p.wd_mode == 0 && !(sizeof(W) == 2 && p.sr);
   if constexpr (MAXV <= 4) {
     if (walk_enabled && simple_opt) {
       p.chunk_done = (uint8_t*) (ws + L.done);
-      // occupancy beats entries in flight per warp (1 M distinct rows: 2 x 4 CTAs 392 us, 4 x 3 CTAs 436 us, 8 x 2 CTAs 488 us).
+      // entries in flight per warp vs CTAs per SM. One H100, 4 tables x 262144 distinct ids (tools/kernel_bench.py): =1 775 us,
+      // =2 732 us, =3 814 us; =1 stays the default until the choice is re-measured on the whole step.
       // TRB_BWD_WALK=1 (default): D <= 128 -> 2 entries / 4 CTAs per SM; =3: 4 entries / 3 CTAs; =2: 4 entries / 2 CTAs
       if (walk_enabled == 2) tbe_bwd_walk_kernel<W, G, MAXV, 2><<<(unsigned) blocks, threads, 0, stream>>>(p);
       else if (walk_enabled == 3 && MAXV == 1) tbe_bwd_walk_kernel<W, G, MAXV, 3, 4><<<(unsigned) blocks, threads, 0, stream>>>(p);   // 4 entries in flight, 3 CTAs / SM
@@ -1021,7 +1019,7 @@ static int run_bwd(TbeBwdParams& p, char* ws, cudaStream_t stream) {
   const size_t smem = (size_t) kLongWarps * p.max_dim * sizeof(float);
   if (smem > 48 * 1024)
     TRB_CUDA(cudaFuncSetAttribute(tbe_bwd_span_long_kernel<W, MAXV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem));
-  tbe_bwd_span_long_kernel<W, MAXV><<<148, kLongWarps * 32, smem, stream>>>(p);
+  tbe_bwd_span_long_kernel<W, MAXV><<<trb_num_sms(), kLongWarps * 32, smem, stream>>>(p);
   TRB_CHECK_LAUNCH();
   return 0;
 }

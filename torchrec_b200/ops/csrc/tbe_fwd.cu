@@ -1,4 +1,4 @@
-// Table-batched embedding forward kernels (sm_100a).
+// Table-batched embedding forward kernels (sm_90a).
 //
 // One launch covers every feature of a table group: bag n = f * B + b gathers rows
 // indices[offsets[n] : offsets[n+1]] of feature f's table, pools them (SUM / MEAN, optional
@@ -149,8 +149,8 @@ __global__ void __launch_bounds__(256) tbe_pooled_fwd_chunk_kernel(const TbeFwdP
   const int64_t e_end = last_end;
 
   // ---- fast path: every bag of the chunk holds exactly ONE id (one-hot features, e.g. Criteo) and the 32 samples go to
-  // one destination rank: no bag bookkeeping at all, ~20 instructions per row instead of ~125 (the generic walk below was
-  // instruction-bound at 48 % issue utilisation / 2 TB/s, profiles/ncu_tbe_pooled_fwd_chunk_kernel_r1.md)
+  // one destination rank: no bag bookkeeping at all, ~20 instructions per row instead of ~125 (the generic walk below is
+  // instruction-bound)
   {
     const bool unit = lane >= nb || (my_end - my_start) == 1;
     const int s0 = b0 / p.B_local;

@@ -1,4 +1,4 @@
-// Gradient of the pooled table-batched lookup w.r.t. the per-sample weights (sm_100a):
+// Gradient of the pooled table-batched lookup w.r.t. the per-sample weights (sm_90a):
 //     d psw[i] = < grad_out[bag(i)][cols of f] , W[idx[i]] >     (x 1/L for MEAN pooling)
 // One warp per bag keeps the bag's gradient row in registers and streams the bag's table rows through it;
 // gradient rows may live on NVLink peers (same addressing as the fused backward). Must run BEFORE the fused

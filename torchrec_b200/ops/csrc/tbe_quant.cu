@@ -1,13 +1,11 @@
-// Inference table-batched lookup over quantized rows (sm_100a).
+// Inference table-batched lookup over quantized rows (sm_90a).
 //
 // Row formats (per table, mixed freely inside one launch):
 //   FMT_FP32 / FMT_FP16 / FMT_BF16 : plain rows
 //   FMT_INT8 / FMT_INT4 / FMT_INT2 : row-wise quantized, fused tail [scale fp16][bias fp16] after the packed
 //                                    values (layout of fbgemm FloatOrHalfToFusedNBitRowwiseQuantizedSBHalf,
 //                                    reference quant/embedding_modules.py:206-283)
-//   FMT_FP8_BLOCK                  : B200-native format: e4m3 values + one fp16 scale per 32-element block
-//                                    ([D bytes][D/32 x fp16]) — the block-scaled layout tensor cores consume, so
-//                                    the same table bytes can feed fp8 GEMMs later without re-quantising
+//   FMT_FP8_BLOCK                  : e4m3 values + one fp16 scale per 32-element block ([D bytes][D/32 x fp16])
 // One warp per bag; lane l dequantises elements 4l..4l+3 (+128k), accumulates in fp32, writes fp32/bf16/fp16.
 // Parity: IntNBitTableBatchedEmbeddingBagsCodegen forward (reference quant_embedding_kernel.py:247-711).
 #include "common.cuh"

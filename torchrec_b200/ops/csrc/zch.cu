@@ -85,7 +85,9 @@ __global__ void __launch_bounds__(256) zch_probe_kernel(const ZchParams p) {
           break;
         }
         if (p.readonly) continue;
-        const int seen = p.metadata[s];
+        // the owner's hour is stamped BEFORE its claim (below): read it after the identity, never older than that claim
+        __threadfence();
+        const int seen = *reinterpret_cast<volatile int*>(p.metadata + s);
         if (p.policy == 1 && p.ttl >= 0 && cand < 0 && seen + p.ttl < p.now) { cand = s; cand_owner = cur; cand_probe = q; }
         if (p.policy == 2 && seen < p.now && seen < lru_seen) { lru_seen = seen; lru_slot = s; lru_owner = cur; }
       }
@@ -93,6 +95,10 @@ __global__ void __launch_bounds__(256) zch_probe_kernel(const ZchParams p) {
       bool lru_pick = false;
       if (cand < 0 && p.policy == 2 && lru_slot >= 0 && lru_retries < 8) { cand = lru_slot; cand_owner = lru_owner; lru_pick = true; ++lru_retries; }
       if (cand < 0) break;
+      // stamp the hour first: a slot claimed in this batch must not look expired / least recently seen to the other threads of the
+      // batch (they would take it over again). A lost claim leaves `now` on a slot its winner stamps with `now` as well.
+      *reinterpret_cast<volatile int*>(p.metadata + cand) = p.now;
+      __threadfence();
       const unsigned long long prev = atomicCAS(p.identities + cand, cand_owner, (unsigned long long) id);
       if (prev == cand_owner) {
         res = cand;

@@ -1,8 +1,8 @@
-"""Dense-arch kernels front-end: fused Linear+bias+activation (tcgen05/TMEM GEMM), dot interaction.
+"""Dense-arch kernels front-end: fused Linear+bias+activation (wgmma GEMM), dot interaction.
 
-``set_dense_backend("tcgen05")`` routes ``Perceptron`` layers and ``InteractionArch`` through the
-hand-written sm_100a kernels in ``csrc/gemm_tcgen05.cu`` / ``csrc/interaction.cu`` (bf16 operands,
-fp32 accumulation in TMEM, bias+ReLU fused in the epilogue). ``"torch"`` keeps stock PyTorch ops
+``set_dense_backend("wgmma")`` routes ``Perceptron`` layers and ``InteractionArch`` through the
+hand-written sm_90a kernels in ``csrc/gemm_wgmma.cu`` / ``csrc/interaction.cu`` (bf16 operands,
+fp32 accumulation in registers, bias+ReLU fused in the epilogue). ``"torch"`` keeps stock PyTorch ops
 (used on CPU and as the numerics oracle).
 """
 from __future__ import annotations
@@ -22,9 +22,9 @@ ACT_NONE, ACT_RELU, ACT_SIGMOID = 0, 1, 2
 
 def set_dense_backend(name: str) -> None:
     global _BACKEND
-    if name not in ("torch", "tcgen05"):
+    if name not in ("torch", "wgmma"):
         raise ValueError(name)
-    if name == "tcgen05":
+    if name == "wgmma":
         _lib.lib()
     _BACKEND = name
 
@@ -44,7 +44,7 @@ def fused_act_code(act) -> Optional[int]:
 
 
 def can_fuse(x: torch.Tensor, linear: nn.Linear) -> bool:
-    if _BACKEND != "tcgen05" or not x.is_cuda or x.dim() != 2:
+    if _BACKEND != "wgmma" or not x.is_cuda or x.dim() != 2:
         return False
     # TMA needs 16-byte aligned row pitches: K and N multiples of 8 bf16 elements
     # N must be a multiple of 8 (16-byte TMA rows of the transposed operands); K is zero-padded to 8
@@ -59,8 +59,8 @@ def linear_act(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tenso
 
 def cast_weights_once(linears) -> Optional[list]:
     """bf16 operands of a stack of fused Linear layers made by ONE kernel (``gemm.cast_pad_weights``); None when the stack is not on
-    the tcgen05 path (the layers then cast their own weights)."""
-    if _BACKEND != "tcgen05" or not linears or len(linears) > 16:
+    the wgmma path (the layers then cast their own weights)."""
+    if _BACKEND != "wgmma" or not linears or len(linears) > 16:
         return None
     ws = [l.weight for l in linears]
     if not all(w.is_cuda and w.dtype == torch.float32 and w.is_contiguous() and l.out_features % 8 == 0 for w, l in zip(ws, linears)):
@@ -74,7 +74,7 @@ def dot_interaction(dense: torch.Tensor, sparse: torch.Tensor) -> torch.Tensor:
     """DLRM pairwise dot interaction. dense [B, D], sparse [B, F, D] ->
     [B, D + (F+1)F/2] = cat(dense, strictly-lower-triangular(X X^T)) with X = [dense; sparse].
     Parity: models/dlrm.py:210-222."""
-    if _BACKEND == "tcgen05" and dense.is_cuda:
+    if _BACKEND == "wgmma" and dense.is_cuda:
         from . import interaction as _inter
 
         if _inter.supported(dense, sparse):

@@ -1,4 +1,4 @@
-"""Python front-end of the hand-written tcgen05 GEMM (``csrc/gemm_tcgen05.cu``).
+"""Python front-end of the hand-written wgmma GEMM (``csrc/gemm_wgmma.cu``).
 
 ``gemm_bf16_tn(a, b)`` computes ``act(alpha * a @ b.T + bias)`` with a ``[M, K]`` and b ``[N, K]``
 (both bf16, K-major). ``LinearActFn`` is the autograd op behind ``Perceptron``:
@@ -33,9 +33,9 @@ def gemm_bf16(a: torch.Tensor, b: torch.Tensor, a_mn: bool = False, b_mn: bool =
               act: int = ACT_NONE, out_dtype: torch.dtype = torch.bfloat16, mask: Optional[torch.Tensor] = None, alpha: float = 1.0,
               out: Optional[torch.Tensor] = None, split_k: int = 1, tile_n: int = 0, mask_bits: Optional[torch.Tensor] = None,
               relu_bits_out: Optional[torch.Tensor] = None, colsum_ws: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """``act(alpha * op(a) @ op(b)^T + bias)`` on the tcgen05 kernel. ``tile_n``: 0 = kernel picks 128 x {64,128,256} tiles,
-    128 / 256 = the caller sized ``split_k`` for that tile width. ``relu_bits_out`` (int32 ``[M, ceil(N / 32)]``, with ``ACT_RELU``):
-    receives one bit per output (> 0); ``mask_bits`` (same layout, with ``ACT_RELU_GRAD``): used instead of re-reading ``mask``.
+    """``act(alpha * op(a) @ op(b)^T + bias)`` on the wgmma kernel (128 x 64 tiles for N <= 64, 128 x 128 otherwise). ``tile_n``: the
+    tile width the caller sized ``split_k`` for (a hint; the kernel's tile depends on N only). ``relu_bits_out`` (int32
+    ``[M, ceil(N / 32)]``, with ``ACT_RELU``): receives one bit per output (> 0); ``mask_bits`` (same layout, with ``ACT_RELU_GRAD``): used instead of re-reading ``mask``.
 
     ``a_mn=False``: a is ``[M, K]`` (K-major);  ``a_mn=True``: a is ``[K, M]`` (consumed MN-major, no transpose copy).
     ``b_mn=False``: b is ``[N, K]``;            ``b_mn=True``: b is ``[K, N]``.
@@ -127,13 +127,10 @@ def _num_sms(device: torch.device) -> int:
 # ReLU layers emit a bit mask of their output for the following layer's masked dgrad (TRB_GEMM_RELU_BITS=0: re-read the activation)
 RELU_BITS = os.environ.get("TRB_GEMM_RELU_BITS", "1") != "0"
 
-# cta_group::2 GEMM (csrc/gemm_tcgen05.cu: gemm_bf16_tcgen05_pair_kernel); the C++ dispatcher reads the same variable
-PAIR_DEFAULT = os.environ.get("TRB_GEMM_PAIR", "1") != "0"
-
 
 def _best_split(tiles: int, K: int, sms: int) -> int:
-    """Split-K factor that fills whole waves of the persistent grid: maximise tiles*s / (ceil(tiles*s / sms) * sms) over splits
-    that keep >= 512 reduction elements each (fewer, fuller waves beat many splits: every split adds a pass of fp32 atomics)."""
+    """Split-K factor that fills whole waves of the grid: maximise tiles*s / (ceil(tiles*s / sms) * sms) over splits that keep
+    >= 512 reduction elements each (fewer, fuller waves beat many splits: every split adds a pass of fp32 atomics)."""
     best, best_score = 1, -1.0
     for s in range(1, max(1, min(64, K // 512)) + 1):
         items = tiles * s
@@ -143,22 +140,15 @@ def _best_split(tiles: int, K: int, sms: int) -> int:
     return best
 
 
+# CTAs of the GEMM kernel resident per SM (csrc/gemm_wgmma.cu: __launch_bounds__(288, 2), a 96 KB operand ring each): one wave of the
+# grid is GEMM_CTAS_PER_SM x SMs tiles
+GEMM_CTAS_PER_SM = 2
+
+
 def _wgrad_plan(n_out: int, n_in: int, batch: int, sms: int) -> "tuple[int, int]":
-    """(split_k, tile_n) of the weight-gradient GEMM ``[n_out, n_in] = gy^T[n_out, batch] . x[batch, n_in]``. 128 x 256 tiles move
-    48 KB of operands per 4.2 MFLOP instead of 32 KB per 2.1 MFLOP: the 1-CTA kernel is bound by L2 -> smem operand traffic, so
-    the wide tile wins whenever the split can still fill the grid. ``TRB_GEMM_SPLIT_WIDE=0`` keeps 128 x 128."""
-    if PAIR_DEFAULT and n_out >= 256 and n_in >= 256:
-        # CTA-pair kernel: 256 x 256 tiles over sms / 2 clusters
-        tiles = ((n_out + 255) // 256) * ((n_in + 255) // 256)
-        s = _best_split(tiles, batch, sms // 2)
-        if tiles * s >= (sms // 2) * 9 // 10:
-            return s, 512
-    m_tiles = (n_out + 127) // 128
-    if n_in % 256 == 0 and os.environ.get("TRB_GEMM_SPLIT_WIDE", "1") != "0":
-        s = _best_split(m_tiles * (n_in // 256), batch, sms)
-        if m_tiles * (n_in // 256) * s >= sms * 9 // 10:
-            return s, 256
-    return _best_split(m_tiles * ((n_in + 127) // 128), batch, sms), 128
+    """(split_k, tile_n) of the weight-gradient GEMM ``[n_out, n_in] = gy^T[n_out, batch] . x[batch, n_in]`` on 128 x 128 tiles."""
+    tiles = ((n_out + 127) // 128) * ((n_in + 127) // 128)
+    return _best_split(tiles, batch, GEMM_CTAS_PER_SM * sms), 128
 
 
 COLSUM_OVERLAP = os.environ.get("TRB_COLSUM_OVERLAP", "1") != "0"
@@ -239,8 +229,8 @@ def cast_pad_weights(weights) -> list:
 
 
 # Bias gradients from the dgrad epilogue of the layer above (``colsum_ws``) instead of a separate column-sum kernel. OFF by default:
-# the K <= 1024 dgrads of the DLRM MLPs are epilogue-bound, and the extra 32 LDS + 64 FADD per lane and slab cost more there (1-GPU step
-# 1.395 -> 1.428 ms) than the separate ``trb_colsum`` kernels do on their side stream. Opt in with TRB_EPI_COLSUM=1 for K >> 1024 stacks.
+# the column sums add shuffles and a named barrier to the epilogue of the dgrad GEMMs on the critical path, while the separate ``trb_colsum``
+# kernels run beside them on their side stream. Opt in with TRB_EPI_COLSUM=1.
 EPI_COLSUM = os.environ.get("TRB_EPI_COLSUM", "0") == "1"
 
 
@@ -251,7 +241,7 @@ def _pad_k(t: torch.Tensor, Kp: int) -> torch.Tensor:
 
 
 class LinearActFn(torch.autograd.Function):
-    """``act(x @ W^T + b)`` on the tcgen05 kernel; bf16 activations, fp32 master weights."""
+    """``act(x @ W^T + b)`` on the wgmma kernel; bf16 activations, fp32 master weights."""
 
     @staticmethod
     def forward(ctx, x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor], act: int, wb: Optional[torch.Tensor] = None) -> torch.Tensor:

@@ -1,4 +1,4 @@
-"""DLRM dot interaction on tcgen05 (``csrc/interaction.cu``)."""
+"""DLRM dot interaction on wgmma tensor cores (``csrc/interaction.cu``)."""
 from __future__ import annotations
 
 import ctypes

@@ -1,5 +1,5 @@
 """Jagged / sparse utility ops (the ``torch.ops.fbgemm.*`` sparse-op surface the reference uses,
-SURVEY §2.4(b)), implemented for both CPU (PyTorch reference) and CUDA (sm_100a kernels in
+SURVEY §2.4(b)), implemented for both CPU (PyTorch reference) and CUDA (sm_90a kernels in
 ``csrc/jagged_ops.cu`` where a hot path needs one; composition of stream-ordered torch ops
 otherwise). No op here performs a hidden host sync unless its output size is data dependent and
 the caller did not pass it.

@@ -4,7 +4,7 @@ SSD behind the HBM row cache (compute kernels KEY_VALUE / DRAM_VIRTUAL_TABLE / S
 Parity: the reference's ``KeyValueEmbedding(Bag)`` / ``ZeroCollisionKeyValueEmbedding(Bag)`` over fbgemm's ``SSDTableBatchedEmbeddingBags``
 (RocksDB / DRAM KV backends, L1 HBM cache + L2 cache; reference distributed/batched_embedding_kernel.py:1917-2508, 3127-3700).
 
-Three tiers, each with the mechanism that fits it on a B200 node:
+Three tiers, each with the mechanism that fits it on an H100 node:
 
     HBM   the row cache of ``UvmCachedEmbeddingBags``: the table-batched lookup / fused optimizer kernels only ever touch cache slots
     store ``store_rows`` row slots per table holding weights + optimizer state,

@@ -1,7 +1,7 @@
 """Inference table-batched embedding over quantized rows (``csrc/tbe_quant.cu``).
 
 Replaces fbgemm ``IntNBitTableBatchedEmbeddingBagsCodegen`` (reference quant/embedding_modules.py:425-442).
-Row formats: FP32, FP16, BF16, INT8 / INT4 / INT2 (row-wise, fused fp16 scale+bias tail) and the B200-native
+Row formats: FP32, FP16, BF16, INT8 / INT4 / INT2 (row-wise, fused fp16 scale+bias tail) and
 block-scaled FP8 (e4m3 + one fp16 scale per 32 elements)."""
 from __future__ import annotations
 

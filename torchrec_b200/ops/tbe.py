@@ -1,11 +1,11 @@
 """Table-batched embedding (TBE) engine: one flat weight buffer for many tables, a single-launch
 pooled / sequence forward and a fused exact backward+optimizer.
 
-B200-native replacement for FBGEMM's ``SplitTableBatchedEmbeddingBagsCodegen`` /
+H100-native replacement for FBGEMM's ``SplitTableBatchedEmbeddingBagsCodegen`` /
 ``DenseTableBatchedEmbeddingBagsCodegen`` as used by the reference wrappers
 (torchrec/distributed/batched_embedding_kernel.py:2915-3124, 3703-3826, 4636-4691).
 
-CUDA tensors always run the sm_100a kernels in ``csrc/tbe_fwd.cu`` / ``csrc/tbe_bwd.cu``; CPU
+CUDA tensors always run the sm_90a kernels in ``csrc/tbe_fwd.cu`` / ``csrc/tbe_bwd.cu``; CPU
 tensors run the PyTorch reference implementation in this file (also the numerics oracle of the
 GPU tests).
 """

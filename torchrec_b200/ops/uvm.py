@@ -3,7 +3,7 @@
 Parity: fbgemm's UVM + LRU/LFU cache inside SplitTableBatchedEmbeddingBagsCodegen (``prefetch`` / ``flush`` /
 ``cache_load_factor``; reference call sites distributed/embedding_lookup.py:714-767, batched_embedding_kernel.py).
 
-Design (B200-first, not a port of the 32-way set-associative lxu cache): the table-batched kernels ALWAYS run on a
+Design (GPU-first, not a port of the 32-way set-associative lxu cache): the table-batched kernels ALWAYS run on a
 device-resident cache table and see *slot* ids; a direct map ``slot_of_row`` (int32 per row, in HBM: 4 B/row) translates
 ids -> slots, so the cache is fully associative and there are no conflict misses. ``prefetch`` (on a side stream, one
 batch ahead) makes every id of the batch resident: victims are the least-recently / least-frequently used slots, their

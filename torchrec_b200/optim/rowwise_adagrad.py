@@ -2,7 +2,7 @@
 
 One accumulator per embedding row: ``sum[r] += mean(grad[r]^2)``, ``w[r] -= lr * grad[r] /
 (sqrt(sum[r]) + eps)``. Used (a) as the tag class for ``apply_optimizer_in_backward`` — the sharded
-tables then run the fused sm_100a kernel — and (b) as the CPU golden implementation in tests.
+tables then run the fused sm_90a kernel — and (b) as the CPU golden implementation in tests.
 """
 from typing import Any, Dict, Iterable, List, Optional
 

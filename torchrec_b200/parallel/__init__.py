@@ -1,4 +1,4 @@
-"""Distributed runtime: model parallelism for embedding tables on B200 (one process per GPU, NCCL + NVLink peer memory).
+"""Distributed runtime: model parallelism for embedding tables on H100 (one process per GPU, NCCL + NVLink peer memory).
 
 Mirrors the top-level surface of ``torchrec/distributed/__init__.py``; also importable as ``torchrec_b200.distributed``.
 

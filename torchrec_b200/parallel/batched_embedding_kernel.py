@@ -3,12 +3,12 @@
 Reference: ``torchrec/distributed/batched_embedding_kernel.py`` - ``BaseBatchedEmbeddingBag`` :2915-3124, ``BatchedFusedEmbeddingBag`` :3703-3826,
 ``BatchedDenseEmbeddingBag`` :4636, the sequence twins :1729-2913, ``EmbeddingFusedOptimizer`` :1195-1624 and the key-value (virtual table) variants
 :1917-2508 / :3127-3700. The reference builds FBGEMM ``SplitTableBatchedEmbeddingBagsCodegen`` / ``DenseTableBatchedEmbeddingBagsCodegen`` / SSD TBEs; here
-every variant is the same hand-written sm_100a kernel family (``ops/csrc/tbe_fwd.cu`` / ``tbe_bwd.cu`` through ``ops/tbe.py``) configured by
+every variant is the same hand-written sm_90a kernel family (``ops/csrc/tbe_fwd.cu`` / ``tbe_bwd.cu`` through ``ops/tbe.py``) configured by
 
 * the optimizer (``OptimType.NONE`` -> dense gradient for DDP / an external optimizer, anything else -> fused into the backward),
 * the pooling mode (SUM / MEAN for bags, NONE for sequence lookups),
 * where the rows live: HBM (``fused``), host-mapped (``fused_uvm``) or host rows behind an HBM row cache (``fused_uvm_caching`` and the key-value kernels,
-  ``ops/uvm.py``) - on a 180 GB part the cache variant is what the reference's SSD/DRAM virtual tables become.
+  ``ops/uvm.py``) - on an 80 GB part the cache variant is what the reference's SSD/DRAM virtual tables become.
 """
 from __future__ import annotations
 

@@ -1,6 +1,6 @@
 """Process-group topology helpers (reference torchrec/distributed/comm.py:38-335).
 
-On an 8xB200 HGX box every GPU reaches every peer at full NVLink-5 bandwidth through NVSwitch, so
+On an 8-GPU HGX box every GPU reaches every peer at full NVLink bandwidth through NVSwitch, so
 the "node" (intra) group normally equals the world; the intra/cross split is kept for multi-node
 jobs and for simulating hierarchies on one host (tests override LOCAL_WORLD_SIZE).
 """

@@ -298,7 +298,7 @@ class KJTSplitsAllToAllMeta:
 
 class FusedKJTListSplitsAwaitable(Awaitable[List[KJTListAwaitable]]):
     """ONE size all-to-all for the input dists of ALL pipelined modules (reference :907-1052): the small int exchange is latency bound
-    (~10 us launch + a host sync each), so N modules x S shardings exchanges collapse into one."""
+    (a launch + a host sync each), so N modules x S shardings exchanges collapse into one."""
 
     def __init__(self, requests: List[KJTListSplitsAwaitable[C]], contexts: List[C], pg: Optional[dist.ProcessGroup]) -> None:
         super().__init__()

@@ -5,7 +5,7 @@ Parity: reference ``ShardedBatchedFusedEmbeddingBag`` (batched_embedding_kernel.
 flat TBE weights are ``reduce_scatter_tensor(AVG)``-ed over the replica group and the full buffer is released; a backward
 pre-hook ``all_gather_into_tensor``s it back before the fused backward + optimizer runs. Net effect per step: replicas are
 averaged every step (no periodic ``DMPCollection.sync`` of the weights) and the full copy is not resident while the dense
-part of the model runs — with 180 GB of HBM that is what lets one replica group hold tables sized for the whole group.
+part of the model runs — with 80 GB of HBM per GPU that is what lets one replica group hold tables sized for the whole group.
 
 Here it is a small state machine attached to a ``TableBatchedEmbeddingBags`` (``tbe._fs``) and driven from the lookup
 autograd functions (eager lookup and the fused NVLink lookup + dist)."""

@@ -1,5 +1,5 @@
 """Accessors for the ``fused_params`` dict that sharders pass down to the table-batched kernels (reference
-torchrec/distributed/fused_params.py:43-160). Keys the B200 engine understands: optimizer hyper-parameters (``optimizer``,
+torchrec/distributed/fused_params.py:43-160). Keys the engine understands: optimizer hyper-parameters (``optimizer``,
 ``learning_rate``, ``eps``, ``beta1/2``, ``weight_decay``, ``weight_decay_mode``, ``max_gradient``, ``momentum``), ``stochastic_rounding``,
 ``cache_load_factor`` / ``cache_algorithm`` (UVM caching), ``output_dtype``, plus the inference-side switches below."""
 from __future__ import annotations

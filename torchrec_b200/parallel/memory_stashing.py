@@ -1,7 +1,7 @@
 """Memory stashing: park embedding weights / optimizer state in pinned host memory while they are not needed and bring
 them back just in time (reference torchrec/distributed/memory_stashing.py:38-800).
 
-On a 180 GB B200 this is what lets the *dense* part of a step borrow the HBM of tables it does not touch (e.g. the
+On an 80 GB H100 this is what lets the *dense* part of a step borrow the HBM of tables it does not touch (e.g. the
 optimizer state between its use in the backward of step i and step i+1, or tables of a frozen tower). A stash is an async
 D2H copy on the ``d2h`` stream followed by freeing the device storage in place (``untyped_storage().resize_(0)`` — every
 view, including the table-batched kernel's parameter views, keeps pointing at the same storage object); a restore

@@ -1,14 +1,15 @@
-"""Measured costs of THIS framework's kernels on B200, the numbers the planner's perf model is built from.
+"""Measured costs of THIS framework's kernels on H100, the numbers the planner's perf model is built from.
 
-Every entry names its measurement (all on 8 x B200 HGX boxes of this pool, CUDA events, max over ranks; write-ups under ``profiles/``):
+Measured on one H100 80GB HBM3 (SXM, 700 W power limit) with ``tools/kernel_bench.py`` (CUDA events, L2 flushed, median):
 
-* ``profiles/scaling_r2.md``      isolated NVLink phases at N = 2 and N = 8 (`bench.py --measure-comm`), single-process peer microbenchmark
-                                   (`tools/peer_bench.py`), N = 2 timeline
-* ``profiles/step_breakdown_*``   per-kernel time of the 1-GPU DLRM step
-* ``MEASURED_PEAKS.json``         STREAM-style copy bandwidth of the pool (6.59 TB/s)
+* device-to-device copy: 3015 and 3029 GB/s (read + write bytes) in two runs
+* the lookup kernels at the shape of the busiest rank of an 8-GPU DLRM job (below)
 
-Nothing here is inherited from the reference's A100-era constants (``planner/constants.py:16-45`` there: 2.455 batched-copy factor, 9.22
-data-parallel factor, /10 UVM rule ...): a factor that was never measured on this hardware is not in the model.
+Not measured on H100, because that needs several GPUs of one NVLink domain: the per-peer NVLink rate (the data sheet's 450 GB/s per
+direction stands in for it), how much an all-to-all of W ranks derates it, how much of the transfer the fused lookup + output dist hides
+and how much of the gradient push stays exposed. The model applies no derating and gives no overlap credit for these until they are
+measured. Nothing here is inherited from the reference's A100-era constants (``planner/constants.py:16-45`` there: 2.455 batched-copy
+factor, 9.22 data-parallel factor, /10 UVM rule ...).
 """
 from __future__ import annotations
 
@@ -16,12 +17,13 @@ from typing import Dict
 
 GB = 1024 * 1024 * 1024
 
-# ---- NVLink 5 through NVSwitch ------------------------------------------------------------------------------------------------
-# one direction, one peer, kernel stores == copy engine (fused lookup + dist 680 GB/s, gradient push 670 GB/s, torch peer copy 671 GB/s)
-PEER_STORE_GBPS: float = 670.0
-# all-to-all among W ranks with both directions busy, as a fraction of PEER_STORE_GBPS: W = 2 fused forward 619 / push 630 GB/s;
-# W = 8 fused forward 479 / push 547 GB/s (rank that sends the most). W = 4 was not measured: interpolated.
-ALL_TO_ALL_EFFICIENCY: Dict[int, float] = {1: 1.0, 2: 0.93, 4: 0.85, 8: 0.765}
+COPY_GBPS: float = 3020.0
+
+# ---- NVLink 4 through NVSwitch ------------------------------------------------------------------------------------------------
+# one direction, one peer: H100 SXM data sheet (18 links, 900 GB/s bidirectional)
+PEER_STORE_GBPS: float = 450.0
+# all-to-all among W ranks with both directions busy, as a fraction of PEER_STORE_GBPS (not measured on H100: no derating)
+ALL_TO_ALL_EFFICIENCY: Dict[int, float] = {1: 1.0}
 
 
 def all_to_all_gbps(world_size: int) -> float:
@@ -37,31 +39,23 @@ def all_to_all_gbps(world_size: int) -> float:
 
 
 # ---- table-batched lookup kernels -------------------------------------------------------------------------------------------------
-# forward (tbe_pooled_fwd_chunk, one-hot fp32 rows -> bf16): 4 tables x 262144 rows, 805 MB of row reads + pooled writes in 135 us
-# = 5.96 TB/s of algorithmic bytes against the 6.59 TB/s copy peak (hot rows of small tables are served by the 126 MB L2)
+# forward (tbe_pooled_fwd_chunk, one-hot fp32 rows -> bf16): 4 tables of 20 M rows x 262144 samples, 814 MB of row reads + pooled writes
+# in 297 us = 2.74 TB/s of algorithmic bytes, 90 % of the copy bandwidth
 LOOKUP_FWD_EFFICIENCY: float = 0.90
-# backward (tbe_bwd_chunk + span kernels; keys + radix sort run on an auxiliary stream, off the critical path): 852 k ids x (256 B gradient
-# row + 512 B row read + 512 B row write) = 1.09 GB in 260 + 65 us = 3.4 TB/s
-LOOKUP_BWD_EFFICIENCY: float = 0.51
-# rows narrower than one 512 B warp request: dim 64 / dim 32 forward kernels against dim 128 (ab runs of round 1, same ids)
+# backward (tbe_bwd walk + span kernels, row-wise Adagrad; keys + radix sort run on an auxiliary stream, off the critical path): the same
+# 1.05 M ids, 1.04 M distinct rows: 1.34 GB of gradient rows + row read-modify-writes + row state in 776 us = 1.73 TB/s, 57 %
+LOOKUP_BWD_EFFICIENCY: float = 0.57
+# rows narrower than one 512 B warp request (dim 64 / dim 32) against dim 128: model assumptions, not measured on H100
 HALF_ROW_PENALTY: float = 1.15
 QUARTER_ROW_PENALTY: float = 1.75
 
 
 def fused_overlap(world_size: int) -> float:
     """Share of min(lookup, transfer) that the fused lookup + output-dist kernel hides: T = lookup + transfer - overlap * min(...).
-    W = 2: 110 us lookup, 174 us transfer, 176 us fused -> 0.98; W = 8: 135 / 427 / 490 us -> 0.53."""
-    if world_size <= 2:
-        return 0.98
-    if world_size >= 8:
-        return 0.53
-    return 0.98 + (0.53 - 0.98) * (world_size - 2) / 6.0
+    Not measured on H100: no overlap credit."""
+    return 0.0
 
 
-# gradient dist: captured inside the dense backward graph beside the deferred weight-gradient GEMMs; what stays exposed of the push at
-# W = 8 (348 us standalone, N = 8 step 2.595 -> 2.354 ms when it moved into the graph together with the other overlaps)
-GRAD_PUSH_EXPOSED: float = 0.45
-# device-side barrier, 8 ranks (trb_barrier_kernel): 11 us, three per step
-BARRIER_MS: float = 0.011
-# input dist (kjt_route: lengths + scan + peer write): 35 us for 26 x 32768 one-hot ids, hidden by the pipeline
-INPUT_DIST_MS_PER_MILLION_IDS: float = 0.041
+# gradient dist: captured inside the dense backward graph beside the deferred weight-gradient GEMMs; the share of the push that stays
+# exposed is not measured on H100: all of it
+GRAD_PUSH_EXPOSED: float = 1.0

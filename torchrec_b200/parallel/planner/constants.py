@@ -1,10 +1,9 @@
-"""Hardware model constants of the planner — B200 / NVLink-5 defaults.
+"""Hardware model constants of the planner — H100 SXM / NVLink-4 defaults.
 
 The reference models an A100-era box (HBM 32 GB @ 897 GB/s, 600 GB/s intra-node, 12.5 GB/s cross-node,
-planner/constants.py:16-36); here the defaults describe one 8xB200 HGX node: 180 GB HBM3e per GPU, the
-MEASURED copy bandwidth of this pool (6.6 TB/s, MEASURED_PEAKS.json), 900 GB/s per direction NVLink 5
-through NVSwitch (670 GB/s measured peer store / copy on this pool, all-to-all efficiency by world size in ``calibration.py``) with
-every peer at full bandwidth, 400 Gb/s NICs across nodes. Kernel-cost factors live in ``calibration.py`` with their measurements.
+planner/constants.py:16-36); here the defaults describe one 8xH100 SXM HGX node: 80 GB HBM3 per GPU, the copy bandwidth
+measured on one H100 (``calibration.py``), NVLink 4 through NVSwitch at the data sheet's 450 GB/s per direction with every peer at
+full bandwidth, 400 Gb/s NICs across nodes. Kernel-cost factors live in ``calibration.py`` with their measurements.
 """
 from typing import Dict, Optional
 
@@ -12,9 +11,9 @@ from ..embedding_types import EmbeddingComputeKernel
 
 MAX_SIZE: int = (1 << 63) - 1
 
-from .calibration import HALF_ROW_PENALTY, LOOKUP_BWD_EFFICIENCY, LOOKUP_FWD_EFFICIENCY, PEER_STORE_GBPS, QUARTER_ROW_PENALTY
+from .calibration import COPY_GBPS, HALF_ROW_PENALTY, LOOKUP_BWD_EFFICIENCY, LOOKUP_FWD_EFFICIENCY, PEER_STORE_GBPS, QUARTER_ROW_PENALTY
 
-INTRA_NODE_BANDWIDTH: float = PEER_STORE_GBPS * 1024 * 1024 * 1024 / 1000  # bytes / ms  (measured NVLink-5 peer store, per direction, one peer)
+INTRA_NODE_BANDWIDTH: float = PEER_STORE_GBPS * 1024 * 1024 * 1024 / 1000  # bytes / ms  (NVLink 4, per direction, one peer)
 CROSS_NODE_BANDWIDTH: float = 50 * 1024 * 1024 * 1024 / 1000  # bytes / ms  (400 Gb/s NIC)
 
 MIN_CW_DIM: int = 128
@@ -22,11 +21,11 @@ POOLING_FACTOR: float = 1.0
 
 BIGINT_DTYPE: int = 8
 
-HBM_CAP: int = 180 * 1024 * 1024 * 1024  # 180 GB HBM3e
+HBM_CAP: int = 80 * 1024 * 1024 * 1024  # 80 GB HBM3
 DDR_CAP: int = 2048 * 1024 * 1024 * 1024
 SSD_CAP: int = 16 * 1024 * 1024 * 1024 * 1024
 DDR_MEM_BW: float = 400 * 1024 * 1024 * 1024 / 1000  # bytes / ms
-HBM_MEM_BW: float = 6588 * 1024 * 1024 * 1024 / 1000  # bytes / ms (measured STREAM-style copy)
+HBM_MEM_BW: float = COPY_GBPS * 1024 * 1024 * 1024 / 1000  # bytes / ms (measured device-to-device copy)
 SSD_MEM_BW: float = 7 * 1024 * 1024 * 1024 / 1000
 HBM_TO_DDR_MEM_BW: float = 55 * 1024 * 1024 * 1024 / 1000  # PCIe Gen5 x16
 UVM_CACHING_RATIO: float = 0.2

@@ -187,7 +187,7 @@ class EmbeddingPerfEstimator(ShardEstimator):
                 raise PlannerError(f"No kernel bandwidth for compute device {topo.compute_device}, compute kernel {so.compute_kernel}")
             W, L = topo.world_size, topo.local_world_size
             intra, inter = topo.intra_host_bw, topo.inter_host_bw
-            comm_bw = intra * all_to_all_gbps(W) / PEER_STORE_GBPS if W <= L else inter  # measured all-to-all efficiency of this world size
+            comm_bw = intra * all_to_all_gbps(W) / PEER_STORE_GBPS if W <= L else inter  # all-to-all efficiency of this world size (calibration.py)
             n_row_shards = len({(s.offset[0], s.size[0]) for s in so.shards})
             for shard in so.shards:
                 rows, cols = shard.size

@@ -7,9 +7,9 @@ from .types import HardwarePerfConfig
 
 
 class EmbeddingPerfEstimatorConfig(HardwarePerfConfig):
-    """The planner's default: one 8 x B200 HGX node (``planner/constants.py``)."""
+    """The planner's default: one 8 x H100 HGX node (``planner/constants.py``)."""
 
-    name = "b200"
+    name = "h100"
 
 
 @hbm_mem_bw(K.HBM_MEM_BW)

@@ -29,7 +29,7 @@ from .types import EstimatorPerfCoefficients, HardwarePerfConfig, PerfCoefficien
 
 
 def compute_block_usage_penalty(embedding_dim: int) -> float:
-    """A warp moves 512 B per request: rows narrower than 128 fp32 waste part of it (measured on the TBE forward, ``profiles/``)."""
+    """A warp moves 512 B per request: rows narrower than 128 fp32 waste part of it (``calibration.py``)."""
     if embedding_dim >= K.FULL_BLOCK_EMB_DIM:
         return 1.0
     return K.HALF_BLOCK_PENALTY if embedding_dim >= K.FULL_BLOCK_EMB_DIM // 2 else K.QUARTER_BLOCK_PENALTY
@@ -135,7 +135,7 @@ class TableWiseEvaluator(EmbeddingShardingPerfEvaluator):
         return full
 
     def _overlap(self, ctx: ShardPerfContext, compute: float, comms: float):
-        # fused lookup + output dist: T = lookup + transfer - overlap(W) * min(lookup, transfer)   (measured at W = 2 and W = 8)
+        # fused lookup + output dist: T = lookup + transfer - overlap(W) * min(lookup, transfer)   (calibration.py)
         if ctx.world_size <= ctx.local_world_size and ctx.compute_device == "cuda":
             comms -= min(compute, comms) * CAL.fused_overlap(ctx.world_size)
         return compute, comms
@@ -324,7 +324,7 @@ EmbeddingPerfEstimatorV2 = EmbeddingPerfEstimator  # the annotation-driven estim
 
 
 class EmbeddingPerfEstimatorFactory:
-    """Registry of hardware configs by name: ``EmbeddingPerfEstimatorFactory.create("b200", topology)`` (reference :1779-1936)."""
+    """Registry of hardware configs by name: ``EmbeddingPerfEstimatorFactory.create("h100", topology)`` (reference :1779-1936)."""
 
     _registry: Dict[str, Type[HardwarePerfConfig]] = {}
 
@@ -353,5 +353,5 @@ class EmbeddingPerfEstimatorFactory:
 
 from .config import GB200PerfConfig  # noqa: E402
 
-EmbeddingPerfEstimatorFactory.register("b200", EmbeddingPerfEstimatorConfig)
+EmbeddingPerfEstimatorFactory.register("h100", EmbeddingPerfEstimatorConfig)
 EmbeddingPerfEstimatorFactory.register("gb200", GB200PerfConfig)

@@ -50,7 +50,7 @@ class PerfCoefficientConfig:
 
 class HardwarePerfConfig:
     """Bandwidths of one hardware generation (bytes / ms). Subclass and decorate with ``annotations.hbm_mem_bw(...)`` etc., or pass values here.
-    The defaults are the B200 / NVLink-5 numbers of ``planner/constants.py``."""
+    The defaults are the H100 / NVLink-4 numbers of ``planner/constants.py``."""
 
     name: str = "default"
     hbm_mem_bw: float = K.HBM_MEM_BW
@@ -85,7 +85,7 @@ class HardwarePerfConfig:
         return K.kernel_bw_lookup(compute_device, compute_kernel, self.hbm_mem_bw, self.ddr_mem_bw, self.hbm_to_ddr_mem_bw, caching_ratio, prefetch_pipeline)
 
     def get_comms_bw(self, world_size: int, local_world_size: int) -> float:
-        """Per-direction bytes / ms of one rank inside the job's all-to-all: inside one NVLink domain the measured all-to-all efficiency of
+        """Per-direction bytes / ms of one rank inside the job's all-to-all: inside one NVLink domain the all-to-all efficiency of
         that world size applies to the single-peer rate (``planner/calibration.py``); across hosts the NIC is the limit."""
         if world_size > local_world_size:
             return self.inter_host_bw

@@ -167,7 +167,7 @@ class BasicCommsBandwidths(GeneralizedCommsBandwidth):
 
 
 class Topology:
-    """Cluster description used by the planner. Defaults model 8xB200 per NVLink domain."""
+    """Cluster description used by the planner. Defaults model 8xH100 per NVLink domain."""
 
     def __init__(
         self,
@@ -610,7 +610,7 @@ class TopologyConfigBase(abc.ABC):
 @dataclass(frozen=True)
 class HardwareConfig(TopologyConfigBase):
     """What the hardware offers (detected or looked up per machine type): capacities in bytes, bandwidths in bytes / ms. Subclass with
-    defaults for a machine type (e.g. a B200 HGX host: 180 GB HBM, NVLink 5 intra-host bandwidth)."""
+    defaults for a machine type (e.g. an H100 HGX host: 80 GB HBM, NVLink 4 intra-host bandwidth)."""
 
     hbm_cap_bytes: Optional[int] = None
     ddr_cap_bytes: Optional[int] = None

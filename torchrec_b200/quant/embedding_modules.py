@@ -1,7 +1,7 @@
 """Quantized (inference) embedding collections (reference torchrec/quant/embedding_modules.py:206-1359).
 
 ``EmbeddingBagCollection.from_float(ebc)`` / ``EmbeddingCollection.from_float(ec)`` build modules whose tables are
-row-wise INT8 / INT4 / INT2, FP16 or block-scaled FP8 and run the sm_100a quantized lookup kernel. State-dict layout
+row-wise INT8 / INT4 / INT2, FP16 or block-scaled FP8 and run the sm_90a quantized lookup kernel. State-dict layout
 follows the reference: ``embedding_bags.<table>.weight`` (uint8 rows incl. the fused scale/bias tail)."""
 from __future__ import annotations
 

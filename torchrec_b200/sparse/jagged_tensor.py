@@ -5,7 +5,7 @@ multi-feature ragged batch with key-major values and ``[F x B]`` lengths, lazily
 ``length_per_key`` / ``offset_per_key``, supports variable batch per feature (VBE) through
 ``stride_per_key_per_rank`` + ``inverse_indices``, and exposes the ``dist_*`` hooks the input
 all-to-all uses. The implementation is new: all jagged math goes through
-``torchrec_b200.ops.jagged`` (sm_100a kernels on CUDA, PyTorch on CPU).
+``torchrec_b200.ops.jagged`` (sm_90a kernels on CUDA, PyTorch on CPU).
 """
 from __future__ import annotations
 

@@ -45,7 +45,7 @@ class DataType(Enum):
     UINT8 = "UINT8"
     INT4 = "INT4"
     INT2 = "INT2"
-    FP8 = "FP8"  # block-scaled fp8 (B200-native inference format)
+    FP8 = "FP8"  # block-scaled fp8 (e4m3 + fp16 scale per 32 elements)
 
     def __str__(self) -> str:
         return self.value

@@ -1,8 +1,8 @@
 """Pin the calling process to the CPUs that are NUMA-local to its GPU.
 
-On a two-socket B200 host the GPU hangs off one socket (``nvidia-smi topo -m``: "CPU Affinity 32-63,96-127"). A rank that the
+On a two-socket GPU host the GPU hangs off one socket (``nvidia-smi topo -m``: "CPU Affinity 32-63,96-127"). A rank that the
 scheduler happens to place on the other socket allocates its pinned staging buffers there and every H2D copy crosses the
-socket interconnect; the end-to-end step time then varies run to run (measured: 14.4 M vs 17.9 M samples/s on the same build).
+socket interconnect; the end-to-end step time then varies run to run on the same build.
 The reference leaves placement to the launcher (``torchx`` / ``numactl``); here it is one call."""
 from __future__ import annotations
 

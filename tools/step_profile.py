@@ -1,6 +1,8 @@
-"""Per-kernel CUDA time of the bench train step through torch.profiler (works under torchrun; ncu must not wrap multi-rank
-commands). Prints rank 0's table (us per step) — use it to see what multi-GPU adds over the 1-GPU launch list.
+"""Per-kernel CUDA time of the step ``bench.py`` times, through torch.profiler (works under torchrun; ncu must not wrap multi-rank
+commands). The model is built and prepared as in ``bench.main``: dense CUDA graphs captured (unless ``--cuda-graphs 0``), then
+``init_data_parallel``. Prints rank 0's table (us per step).
 
+    python tools/step_profile.py --gpus 1 [--steps 6]
     torchrun --nproc-per-node 2 tools/step_profile.py --gpus 2 [--steps 6]
 """
 import os
@@ -14,7 +16,6 @@ import bench  # noqa: E402
 
 
 def main() -> None:
-    sys.argv = [sys.argv[0]] + [a for a in sys.argv[1:]]
     args = bench.parse_args()
     world = int(os.environ.get("WORLD_SIZE", "1"))
     rank = int(os.environ.get("RANK", "0"))
@@ -25,10 +26,19 @@ def main() -> None:
         dist.init_process_group("nccl", device_id=device)
     from torchrec_b200.datasets.random import RandomRecDataset
 
-    dmp, opt, keys, hashes, _ = bench.build_ours(args, device, rank, world)
-    dmp.init_data_parallel()
-    ds = RandomRecDataset(keys, args.batch_size, hash_sizes=hashes, ids_per_features=[args.pooling] * 26, num_dense=13, manual_seed=1234 + rank, num_generated_batches=4)
+    torch.manual_seed(0)
+    dmp, opt, keys, hashes, ids_per_feature, num_dense, _backend, _info = bench.build_ours(args, device, rank, world)
+    ds = RandomRecDataset(keys, args.batch_size, hash_sizes=hashes, ids_per_features=ids_per_feature, num_dense=num_dense,
+                          manual_seed=1234 + rank, num_generated_batches=4)
     batches = [b.to(device) for b in ds.batch_generator._generated_batches]
+    inner = getattr(dmp.module, "model", None)
+    if args.cuda_graphs != 0 and hasattr(inner, "capture_dense_graphs"):
+        with torch.no_grad():
+            sample_emb = inner.sparse_arch(batches[0].sparse_features)
+        inner.capture_dense_graphs(batches[0].dense_features, sample_emb)
+        inner.overlap_sparse_dense = bool(args.overlap_sparse)
+        torch.cuda.synchronize()
+    dmp.init_data_parallel()
 
     def step(b):
         opt.zero_grad()

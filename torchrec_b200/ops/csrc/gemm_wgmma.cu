@@ -3,16 +3,30 @@
 // and a fused epilogue (bias, ReLU / sigmoid, ReLU-gradient mask, ReLU bit mask, bias-gradient column sums,
 // bf16 / fp32 store or split-K fp32 reduction).
 //
-// Structure (one 128 x BN output tile per CTA, two CTAs per SM so that one CTA's epilogue overlaps the other's MMAs):
-//   warps 0..3  consumer warpgroup 0   rows [0, 64) of the tile:   4 x wgmma m64nBNk16 per 64-wide k-block
-//   warps 4..7  consumer warpgroup 1   rows [64, 128) of the tile
-//   warp 8      TMA producer           cp.async.bulk.tensor.2d -> smem ring (kStages x (A 128x64, B BNx64))
+// Two kernels share the mainloop and the epilogue:
+//
+// N > 64: gemm_bf16_wgmma_persistent_kernel, 128 x BN tiles (BN = 256; 128 for N <= 128 and for split-K at N <= 256), one CTA per SM walking a static
+// tile list (tile i, i + gridDim.x, ...; consecutive tiles share an A row-block, so the CTAs running at once read the same A rows):
+//   warps 0..3   consumer warpgroup 0   rows [0, 64) of the tile:   4 x wgmma m64nBNk16 per 64-wide k-block
+//   warps 4..7   consumer warpgroup 1   rows [64, 128) of the tile
+//   warps 8..11  producer warpgroup     one thread issues cp.async.bulk.tensor.2d -> smem ring (kStages x (A 128x64, B BNx64))
+// setmaxnreg moves registers from the producer warpgroup (40) to the consumers (232): 128 fp32 accumulators per thread at BN = 256.
+// The producer runs ahead into the next tile's k-blocks while the consumers run the epilogue. A bf16 output without split-K leaves
+// through shared memory: each consumer warpgroup writes its 64 x BN block into a SWIZZLE_128B staging buffer and one thread issues
+// TMA stores (64 x 64 boxes, clipped at M / N by the tensor map), then the warpgroup returns to its MMAs; the staging buffer is
+// reused once the previous tile's stores have read it. fp32 / split-K outputs (and outputs a tensor map cannot describe) are stored
+// from the fragment layout.
+//
+// N <= 64: gemm_bf16_wgmma_kernel, one 128 x 64 tile per CTA and two CTAs per SM (one CTA's epilogue overlaps the other's MMAs);
+// warps 0..7 are the consumers as above, warp 8 the TMA producer.
+//
 // A consumer keeps one wgmma group in flight and releases the previous k-block's slot when it retires.
 //
 // Both operands may be K-major (row-major [rows, K], the natural layout of nn.Linear: x [M,K], weight [N,K]) or
 // MN-major ([K, rows], consumed transposed by wgmma), so dgrad / wgrad need no transpose copies.
 // Replaces the reference's cuBLAS nn.Linear + separate bias/ReLU kernels (modules/mlp.py:18-190).
 #include <cstdlib>
+#include <cstring>
 
 #include "wgmma.cuh"
 
@@ -48,6 +62,7 @@ struct GemmParams {
   // 32-row slab of the bf16 output go to colsum_ws[row0 / 32][n] ([ceil(M / 32), N], deterministic; reduced by
   // trb_colsum_partials). nullptr: not wanted.
   float* colsum_ws;
+  int tma_out;                  // 1: bf16 output through shared memory and TMA stores (persistent kernel, split_k == 1)
 };
 
 __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
@@ -57,7 +72,7 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
 
 template <int BN>
 struct SmemLayout {
-  static constexpr int kStages = BN == 128 ? 3 : 4;   // 96 KB of operand ring: two CTAs per SM
+  static constexpr int kStages = 4;   // 64 KB of operand ring (BN = 64): two CTAs per SM
   static constexpr int kABytes = BLOCK_M * BLOCK_K * 2;
   static constexpr int kBBytes = BN * BLOCK_K * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
@@ -68,8 +83,11 @@ struct SmemLayout {
 
 // Epilogue of one consumer warpgroup: rows [row0, row0 + 64) x cols [n0, n0 + BN) of the output.
 // ACT / BIAS are compile-time so the unrolled loop carries no runtime branches on them.
-template <int BN, int ACT, bool BIAS>
-__device__ __forceinline__ void epilogue_impl(const GemmParams& p, float (&acc)[BN / 2], int row0, int n0, int wq, int lane, float* colsum_s) {
+// STAGED: the bf16 values go to `stage` (BN / 64 SWIZZLE_128B boxes of 64 rows x 64 columns) for a TMA store instead of global memory,
+// and the bias of columns [n0, n0 + BN) is read from `bias_s` (shared memory; a register-resident bias spills at BN = 256).
+template <int BN, int ACT, bool BIAS, bool STAGED>
+__device__ __forceinline__ void epilogue_impl(const GemmParams& p, float (&acc)[BN / 2], int row0, int n0, int wq, int lane, float* colsum_s,
+                                              uint8_t* stage, const float* bias_s) {
   const int q = lane & 3;
   const int rows[2] = {row0 + 16 * wq + (lane >> 2), row0 + 16 * wq + (lane >> 2) + 8};
   const bool row_ok[2] = {rows[0] < p.M, rows[1] < p.M};
@@ -82,7 +100,12 @@ __device__ __forceinline__ void epilogue_impl(const GemmParams& p, float (&acc)[
     const bool col_ok = col < p.N;  // N % 8 == 0: col + 1 < N as well
     float2 b2 = make_float2(0.f, 0.f);
     if constexpr (BIAS) {
-      if (col_ok) b2 = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+      if constexpr (STAGED) {
+        const uint32_t addr = smem_u32(bias_s + 8 * j + 2 * q);
+        asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(b2.x), "=f"(b2.y) : "r"(addr));
+      } else if (col_ok) {
+        b2 = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+      }
     }
     float cs0 = 0.f, cs1 = 0.f;
 #pragma unroll
@@ -113,7 +136,15 @@ __device__ __forceinline__ void epilogue_impl(const GemmParams& p, float (&acc)[
           }
         }
       }
-      if (ok) {
+      if constexpr (STAGED) {
+        // rows / columns outside the output are clipped by the TMA store
+        const uint32_t o = pack_bf16x2(v0, v1);
+        *reinterpret_cast<uint32_t*>(stage + (j >> 3) * 8192 + sw128_offset(16 * wq + (lane >> 2) + 8 * h, 8 * (j & 7) + 2 * q)) = o;
+        if (want_colsum && ok) {
+          cs0 += __uint_as_float(o << 16);
+          cs1 += __uint_as_float(o & 0xffff0000u);
+        }
+      } else if (ok) {
         if (p.split_k > 1) {
           float* o = reinterpret_cast<float*>(p.out) + (int64_t) rows[h] * p.ldo + col;
           atomicAdd(o, v0);
@@ -175,9 +206,10 @@ __device__ __forceinline__ void epilogue_impl(const GemmParams& p, float (&acc)[
   }
 }
 
-template <int BN>
-__device__ __forceinline__ void epilogue(const GemmParams& p, float (&acc)[BN / 2], int row0, int n0, int wq, int lane, float* colsum_s) {
-#define TRB_EPI(A, B) epilogue_impl<BN, A, B>(p, acc, row0, n0, wq, lane, colsum_s)
+template <int BN, bool STAGED>
+__device__ __forceinline__ void epilogue(const GemmParams& p, float (&acc)[BN / 2], int row0, int n0, int wq, int lane, float* colsum_s,
+                                         uint8_t* stage = nullptr, const float* bias_s = nullptr) {
+#define TRB_EPI(A, B) epilogue_impl<BN, A, B, STAGED>(p, acc, row0, n0, wq, lane, colsum_s, stage, bias_s)
   const bool bias = p.bias != nullptr;
   switch (p.act) {
     case ACT_RELU: if (bias) TRB_EPI(ACT_RELU, true); else TRB_EPI(ACT_RELU, false); break;
@@ -195,7 +227,8 @@ __device__ __forceinline__ void mma_kblock(float (&acc)[BN / 2], uint32_t a_addr
     // K-major: +32 B inside the 128 B swizzle row; MN-major: 16 reduction rows x 128 B = 2048 B
     const uint64_t ad = A_MN ? make_smem_desc(a_addr + k * 2048, 8192, 1024) : make_kmajor_desc(a_addr + k * 32);
     const uint64_t bd = B_MN ? make_smem_desc(b_addr + k * 2048, 8192, 1024) : make_kmajor_desc(b_addr + k * 32);
-    if constexpr (BN == 128) wgmma_m64n128k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, ad, bd);
+    if constexpr (BN == 256) wgmma_m64n256k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, ad, bd);
+    else if constexpr (BN == 128) wgmma_m64n128k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, ad, bd);
     else wgmma_m64n64k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, ad, bd);
   }
 }
@@ -289,7 +322,155 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
   wgmma_wait<0>();
   wgmma_fence_regs(acc);
   // (no arrival for the last slot: nothing is loaded after this tile's last k-block)
-  epilogue<BN>(p, acc, m_blk * BLOCK_M + 64 * wg, n_blk * BN, wq, lane, reinterpret_cast<float*>(smem + L::kColsumOffset) + wg * 2 * BN);
+  epilogue<BN, false>(p, acc, m_blk * BLOCK_M + 64 * wg, n_blk * BN, wq, lane, reinterpret_cast<float*>(smem + L::kColsumOffset) + wg * 2 * BN);
+}
+
+constexpr int kPersistentThreads = kConsumerThreads + 128;
+
+template <int BN>
+struct PersistentLayout {
+  static constexpr int kStages = BN == 256 ? 3 : 5;
+  static constexpr int kABytes = BLOCK_M * BLOCK_K * 2;
+  static constexpr int kBBytes = BN * BLOCK_K * 2;
+  static constexpr int kStageBytes = kABytes + kBBytes;
+  static constexpr int kOutOffset = kStages * kStageBytes;             // [2 warpgroups][64 rows x BN] bf16 staging of the TMA store
+  static constexpr int kOutBytes = 64 * BN * 2;                        // per warpgroup
+  static constexpr int kColsumOffset = kOutOffset + 2 * kOutBytes;     // [2 warpgroups][2 slabs][BN] fp32
+  static constexpr int kBiasOffset = kColsumOffset + 4 * BN * 4;      // [2 warpgroups][BN] fp32 bias of the tile's columns
+  static constexpr int kBarOffset = kBiasOffset + 2 * BN * 4;
+  static constexpr int kTotal = kBarOffset + 2 * kStages * 8;
+  static_assert(kTotal + 1024 <= 227 * 1024, "shared memory of one CTA per SM");
+};
+
+__device__ __forceinline__ void warpgroup_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
+
+// TMA_OUT: bf16 output through the staging buffer and TMA stores (p.tma_out); otherwise stores from the fragment layout.
+template <int BN, bool A_MN, bool B_MN, bool TMA_OUT>
+__global__ void __launch_bounds__(kPersistentThreads, 1)
+gemm_bf16_wgmma_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                                  const __grid_constant__ CUtensorMap tmap_out, const GemmParams p) {
+  using L = PersistentLayout<BN>;
+  constexpr int kStages = L::kStages;
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t) 1023);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::kBarOffset);
+  uint64_t* empty_bar = full_bar + kStages;
+
+  const int warp_idx = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < kStages; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], 2);  // one arrival per consumer warpgroup
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  const int m_tiles = (p.M + BLOCK_M - 1) / BLOCK_M;
+  const int n_tiles = (p.N + BN - 1) / BN;
+  const int k_blocks_total = (p.K + BLOCK_K - 1) / BLOCK_K;
+  const int splits = p.split_k > 1 ? p.split_k : 1;
+  const int kb_per_split = (k_blocks_total + splits - 1) / splits;
+  const int mn_tiles = m_tiles * n_tiles;
+  const int items = mn_tiles * splits;
+
+  if (warp_idx >= kConsumerThreads / 32) {
+    // ================= TMA producer warpgroup =================
+    setmaxnreg_dec<40>();
+    if (warp_idx == kConsumerThreads / 32 && lane == 0) {
+      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmap_a)) : "memory");
+      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmap_b)) : "memory");
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int item = blockIdx.x; item < items; item += gridDim.x) {
+        const int mn = item % mn_tiles, ks = item / mn_tiles;
+        const int m_blk = mn / n_tiles, n_blk = mn % n_tiles;
+        const int kb0 = ks * kb_per_split, kb1 = min(k_blocks_total, kb0 + kb_per_split);
+        for (int kb = kb0; kb < kb1; ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1);
+          uint8_t* sa = smem + stage * L::kStageBytes;
+          uint8_t* sb = sa + L::kABytes;
+          mbar_arrive_expect_tx(&full_bar[stage], L::kStageBytes);
+          if constexpr (A_MN) {
+#pragma unroll
+            for (int h = 0; h < BLOCK_M / 64; ++h) tma_load_2d(&tmap_a, &full_bar[stage], sa + h * 8192, m_blk * BLOCK_M + 64 * h, kb * BLOCK_K);
+          } else {
+            tma_load_2d(&tmap_a, &full_bar[stage], sa, kb * BLOCK_K, m_blk * BLOCK_M);
+          }
+          if constexpr (B_MN) {
+#pragma unroll
+            for (int h = 0; h < BN / 64; ++h) tma_load_2d(&tmap_b, &full_bar[stage], sb + h * 8192, n_blk * BN + 64 * h, kb * BLOCK_K);
+          } else {
+            tma_load_2d(&tmap_b, &full_bar[stage], sb, kb * BLOCK_K, n_blk * BN);
+          }
+          if (++stage == kStages) { stage = 0; phase ^= 1; }
+        }
+      }
+    }
+    return;
+  }
+
+  // ================= consumers =================
+  setmaxnreg_inc<232>();
+  const int wg = warp_idx >> 2;  // rows [64 wg, 64 wg + 64) of the tile
+  const int wq = warp_idx & 3;
+  const bool leader = (threadIdx.x & 127) == 0;
+  const uint32_t a_off = (uint32_t) wg * 8192u;
+  uint8_t* out_stage = smem + L::kOutOffset + wg * L::kOutBytes;
+  float* colsum_s = reinterpret_cast<float*>(smem + L::kColsumOffset) + wg * 2 * BN;
+  float* bias_s = reinterpret_cast<float*>(smem + L::kBiasOffset) + wg * BN;
+  int stage = 0;
+  uint32_t phase = 0;
+  float acc[BN / 2];
+  for (int item = blockIdx.x; item < items; item += gridDim.x) {
+    const int mn = item % mn_tiles, ks = item / mn_tiles;
+    const int m_blk = mn / n_tiles, n_blk = mn % n_tiles;
+    const int kb0 = ks * kb_per_split, kb1 = min(k_blocks_total, kb0 + kb_per_split);
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    int prev_stage = stage;
+    for (int kb = kb0; kb < kb1; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t a_addr = smem_u32(smem + stage * L::kStageBytes) + a_off;
+      const uint32_t b_addr = smem_u32(smem + stage * L::kStageBytes + L::kABytes);
+      wgmma_fence();
+      mma_kblock<BN, A_MN, B_MN>(acc, a_addr, b_addr);
+      wgmma_commit();
+      wgmma_wait<1>();  // the previous k-block's wgmmas retired: its smem slot is free
+      wgmma_fence_regs(acc);
+      if (kb > kb0 && leader) mbar_arrive(&empty_bar[prev_stage]);
+      prev_stage = stage;
+      if (++stage == kStages) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc);
+    if (leader) mbar_arrive(&empty_bar[prev_stage]);  // the producer may already be loading the next tile
+    const int row0 = m_blk * BLOCK_M + 64 * wg, n0 = n_blk * BN;
+    if constexpr (TMA_OUT) {
+      if (leader) tma_store_wait_read();  // the previous tile's stores have read the staging buffer
+      warpgroup_sync(wg);                 // ... and every warp is past the previous epilogue (colsum_s / bias_s are free as well)
+      if (p.bias != nullptr) {
+        for (int c = threadIdx.x & 127; c < BN; c += 128) bias_s[c] = n0 + c < p.N ? p.bias[n0 + c] : 0.f;
+        warpgroup_sync(wg);
+      }
+      epilogue<BN, true>(p, acc, row0, n0, wq, lane, colsum_s, out_stage, bias_s);
+      fence_proxy_async();
+      warpgroup_sync(wg);
+      if (leader && row0 < p.M) {
+#pragma unroll
+        for (int b = 0; b < BN / 64; ++b)
+          if (n0 + 64 * b < p.N) tma_store_2d(&tmap_out, out_stage + b * 8192, n0 + 64 * b, row0);
+        tma_store_commit();
+      }
+    } else {
+      warpgroup_sync(wg);  // every warp is past the previous epilogue: colsum_s is free
+      epilogue<BN, false>(p, acc, row0, n0, wq, lane, colsum_s);
+    }
+  }
+  if constexpr (TMA_OUT) {
+    if (leader) tma_store_wait_all();
+  }
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
@@ -317,6 +498,26 @@ int make_tmap(CUtensorMap* map, const void* ptr, int64_t rows, int64_t K, int64_
   CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? 0 : -11;
+}
+
+template <int BN, bool A_MN, bool B_MN>
+int launch_gemm_persistent(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to, const GemmParams& p, cudaStream_t stream) {
+  constexpr int smem_bytes = PersistentLayout<BN>::kTotal + 1024;
+  static bool configured = false;
+  if (!configured) {
+    TRB_CUDA(cudaFuncSetAttribute(gemm_bf16_wgmma_persistent_kernel<BN, A_MN, B_MN, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
+    TRB_CUDA(cudaFuncSetAttribute(gemm_bf16_wgmma_persistent_kernel<BN, A_MN, B_MN, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
+    configured = true;
+  }
+  const int64_t items = (int64_t) ((p.M + BLOCK_M - 1) / BLOCK_M) * ((p.N + BN - 1) / BN) * (p.split_k > 1 ? p.split_k : 1);
+  if (items > 0x7fffffff) return -12;
+  const int grid = (int) (items < trb_num_sms() ? items : trb_num_sms());
+  if (p.tma_out)
+    gemm_bf16_wgmma_persistent_kernel<BN, A_MN, B_MN, true><<<grid, kPersistentThreads, smem_bytes, stream>>>(ta, tb, to, p);
+  else
+    gemm_bf16_wgmma_persistent_kernel<BN, A_MN, B_MN, false><<<grid, kPersistentThreads, smem_bytes, stream>>>(ta, tb, to, p);
+  TRB_CHECK_LAUNCH();
+  return 0;
 }
 
 template <int BN, bool A_MN, bool B_MN>
@@ -351,9 +552,18 @@ static int gemm_dispatch(const void* A, int64_t lda, const void* B, int64_t ldb,
     if (rc) return rc;
     return launch_gemm<64, A_MN, B_MN>(ta, tb, p, stream);
   }
-  rc = B_MN ? make_tmap(&tb, B, p.K, p.N, ldb, 64, 64) : make_tmap(&tb, B, p.N, p.K, ldb, 128);
+  // split-K items of narrow outputs stay 128 wide: the split plans (gemm.py _wgrad_plan) fill the grid with 128 x 128 items, and at
+  // N <= 256 one 128 x 256 item per (m, n) block would leave half the SMs idle
+  const int bn = (p.N <= 128 || (p.split_k > 1 && p.N <= 256)) ? 128 : 256;
+  rc = B_MN ? make_tmap(&tb, B, p.K, p.N, ldb, 64, 64) : make_tmap(&tb, B, p.N, p.K, ldb, bn);
   if (rc) return rc;
-  return launch_gemm<128, A_MN, B_MN>(ta, tb, p, stream);
+  // bf16 output without split-K: TMA stores of 64 x 64 boxes (needs a 16 B aligned base and row pitch)
+  CUtensorMap to;
+  memset(&to, 0, sizeof(to));
+  p.tma_out = !p.out_f32 && p.split_k == 1 && reinterpret_cast<uintptr_t>(p.out) % 16 == 0 && p.ldo % 8 == 0 &&
+              make_tmap(&to, p.out, p.M, p.N, p.ldo, 64, 64) == 0;
+  if (bn == 128) return launch_gemm_persistent<128, A_MN, B_MN>(ta, tb, to, p, stream);
+  return launch_gemm_persistent<256, A_MN, B_MN>(ta, tb, to, p, stream);
 }
 
 TRB_API int trb_gemm_bf16_ex2(const void* A, int64_t lda, int a_mn, const void* B, int64_t ldb, int b_mn, void* out, int64_t ldo, int out_f32, int M,
@@ -380,7 +590,7 @@ TRB_API int trb_gemm_bf16_ex2(const void* A, int64_t lda, int a_mn, const void* 
 }
 
 // colsum_ws: fp32 [ceil(M / 32), N] or nullptr, see GemmParams (bf16 output without split-K only: -14 otherwise).
-// tile_n: tile-width hint of the caller's split-K plan; this kernel has one tile shape per N (128 x 64 or 128 x 128).
+// tile_n: tile-width hint of the caller's split-K plan; the tile shape depends on N only (128 x 64, 128 x 128 or 128 x 256).
 TRB_API int trb_gemm_bf16_ex3(const void* A, int64_t lda, int a_mn, const void* B, int64_t ldb, int b_mn, void* out, int64_t ldo, int out_f32, int M,
                               int N, int K, const float* bias, int act, const void* mask, int64_t ld_mask, float alpha, int split_k, int tile_n,
                               const void* mask_bits, void* relu_bits_out, int64_t ld_bits, float* colsum_ws, cudaStream_t stream) {
@@ -402,6 +612,7 @@ TRB_API int trb_gemm_bf16_ex3(const void* A, int64_t lda, int a_mn, const void* 
   p.relu_bits_out = reinterpret_cast<uint32_t*>(relu_bits_out);
   p.ld_bits = ld_bits;
   p.colsum_ws = colsum_ws;
+  p.tma_out = 0;
   if ((mask_bits != nullptr || relu_bits_out != nullptr) && ld_bits * 32 < N) return -12;
   if (split_k > 1) {
     if (!out_f32 || bias != nullptr || act != ACT_NONE) return -13;  // split-K only for plain fp32 accumulation

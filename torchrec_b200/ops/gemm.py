@@ -33,8 +33,9 @@ def gemm_bf16(a: torch.Tensor, b: torch.Tensor, a_mn: bool = False, b_mn: bool =
               act: int = ACT_NONE, out_dtype: torch.dtype = torch.bfloat16, mask: Optional[torch.Tensor] = None, alpha: float = 1.0,
               out: Optional[torch.Tensor] = None, split_k: int = 1, tile_n: int = 0, mask_bits: Optional[torch.Tensor] = None,
               relu_bits_out: Optional[torch.Tensor] = None, colsum_ws: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """``act(alpha * op(a) @ op(b)^T + bias)`` on the wgmma kernel (128 x 64 tiles for N <= 64, 128 x 128 otherwise). ``tile_n``: the
-    tile width the caller sized ``split_k`` for (a hint; the kernel's tile depends on N only). ``relu_bits_out`` (int32
+    """``act(alpha * op(a) @ op(b)^T + bias)`` on the wgmma kernels: 128 x 64 tiles for N <= 64 (two CTAs per SM), otherwise a
+    persistent kernel (one CTA per SM) on 128 x 128 tiles for N <= 128 and 128 x 256 tiles above (128 x 128 for split-K up to N = 256).
+    ``tile_n``: the tile width the caller sized ``split_k`` for (a hint; the kernel's tile depends on N and split-K only). ``relu_bits_out`` (int32
     ``[M, ceil(N / 32)]``, with ``ACT_RELU``): receives one bit per output (> 0); ``mask_bits`` (same layout, with ``ACT_RELU_GRAD``): used instead of re-reading ``mask``.
 
     ``a_mn=False``: a is ``[M, K]`` (K-major);  ``a_mn=True``: a is ``[K, M]`` (consumed MN-major, no transpose copy).
@@ -140,13 +141,14 @@ def _best_split(tiles: int, K: int, sms: int) -> int:
     return best
 
 
-# CTAs of the GEMM kernel resident per SM (csrc/gemm_wgmma.cu: __launch_bounds__(288, 2), a 96 KB operand ring each): one wave of the
-# grid is GEMM_CTAS_PER_SM x SMs tiles
+# 128 x 128 work items per SM in one wave of the GEMM grid: the persistent kernel (csrc/gemm_wgmma.cu) runs one CTA per SM on 128 x 256
+# tiles, i.e. two 128 x 128 items, and the 128 x 64 kernel of N <= 64 runs two CTAs per SM
 GEMM_CTAS_PER_SM = 2
 
 
 def _wgrad_plan(n_out: int, n_in: int, batch: int, sms: int) -> "tuple[int, int]":
-    """(split_k, tile_n) of the weight-gradient GEMM ``[n_out, n_in] = gy^T[n_out, batch] . x[batch, n_in]`` on 128 x 128 tiles."""
+    """(split_k, tile_n) of the weight-gradient GEMM ``[n_out, n_in] = gy^T[n_out, batch] . x[batch, n_in]``, sized in 128 x 128 items
+    (GEMM_CTAS_PER_SM x SMs of them fill one wave, also when the kernel runs them as 128 x 256 tiles)."""
     tiles = ((n_out + 127) // 128) * ((n_in + 127) // 128)
     return _best_split(tiles, batch, GEMM_CTAS_PER_SM * sms), 128
 

@@ -168,9 +168,10 @@ def test_psw_grad_matches_reference():
 @pytest.mark.gpu
 @pytest.mark.parametrize("opt", [T.OptimType.EXACT_SGD, T.OptimType.EXACT_ROWWISE_ADAGRAD])
 @pytest.mark.parametrize("dim,gdtype", [(128, torch.bfloat16), (64, torch.float32), (256, torch.float32)])
-def test_fused_backward_unique_rows_fast_path(opt, dim, gdtype):
-    """Large tables -> (almost) all ids distinct: exercises the one-hot forward and the unique-rows backward fast paths,
-    mixed with a tiny table whose chunks take the generic walk."""
+def test_fused_backward_walk_kernel_mostly_distinct_ids(opt, dim, gdtype):
+    """Large tables -> (almost) all ids distinct: exercises the one-hot forward and the multi-row backward walk
+    (tbe_bwd_walk_kernel, both of its shapes: D <= 128 and D <= 512), mixed with a tiny table whose duplicate ids
+    take the generic walk."""
     dev = torch.device("cuda:0")
     specs = [(200_000, dim), (7, dim), (150_000, dim)]
     fmap = [0, 1, 2]

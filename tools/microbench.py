@@ -125,7 +125,6 @@ def bench_tbe(rows_per_table=40_000_000, n_tables=8):
 
 if __name__ == "__main__":
     which = sys.argv[1:] or ["gemm", "interaction", "tbe"]
-    print(f"env: TRB_INTERACTION_LEGACY={os.environ.get('TRB_INTERACTION_LEGACY')}\n")
     for w in which:
         {"gemm": bench_gemm, "interaction": bench_interaction, "tbe": bench_tbe, "colsum": bench_colsum, "gemmx": bench_gemmx}[w]()
         print()

@@ -25,7 +25,6 @@
 // Both operands may be K-major (row-major [rows, K], the natural layout of nn.Linear: x [M,K], weight [N,K]) or
 // MN-major ([K, rows], consumed transposed by wgmma), so dgrad / wgrad need no transpose copies.
 // Replaces the reference's cuBLAS nn.Linear + separate bias/ReLU kernels (modules/mlp.py:18-190).
-#include <cstdlib>
 #include <cstring>
 
 #include "wgmma.cuh"
@@ -566,34 +565,12 @@ static int gemm_dispatch(const void* A, int64_t lda, const void* B, int64_t ldb,
   return launch_gemm_persistent<256, A_MN, B_MN>(ta, tb, to, p, stream);
 }
 
-TRB_API int trb_gemm_bf16_ex2(const void* A, int64_t lda, int a_mn, const void* B, int64_t ldb, int b_mn, void* out, int64_t ldo, int out_f32, int M,
-                              int N, int K, const float* bias, int act, const void* mask, int64_t ld_mask, float alpha, int split_k, int tile_n,
-                              const void* mask_bits, void* relu_bits_out, int64_t ld_bits, cudaStream_t stream);
-
-TRB_API int trb_gemm_bf16_ex(const void* A, int64_t lda, int a_mn, const void* B, int64_t ldb, int b_mn, void* out, int64_t ldo, int out_f32, int M,
-                             int N, int K, const float* bias, int act, const void* mask, int64_t ld_mask, float alpha, int split_k, int tile_n,
-                             cudaStream_t stream) {
-  return trb_gemm_bf16_ex2(A, lda, a_mn, B, ldb, b_mn, out, ldo, out_f32, M, N, K, bias, act, mask, ld_mask, alpha, split_k, tile_n, nullptr, nullptr, 0,
-                           stream);
-}
-
-// mask_bits / relu_bits_out: int32 [M, ld_bits] bit matrices (bit n % 32 of word n / 32), see GemmParams
-TRB_API int trb_gemm_bf16_ex3(const void* A, int64_t lda, int a_mn, const void* B, int64_t ldb, int b_mn, void* out, int64_t ldo, int out_f32, int M,
-                              int N, int K, const float* bias, int act, const void* mask, int64_t ld_mask, float alpha, int split_k, int tile_n,
-                              const void* mask_bits, void* relu_bits_out, int64_t ld_bits, float* colsum_ws, cudaStream_t stream);
-
-TRB_API int trb_gemm_bf16_ex2(const void* A, int64_t lda, int a_mn, const void* B, int64_t ldb, int b_mn, void* out, int64_t ldo, int out_f32, int M,
-                              int N, int K, const float* bias, int act, const void* mask, int64_t ld_mask, float alpha, int split_k, int tile_n,
-                              const void* mask_bits, void* relu_bits_out, int64_t ld_bits, cudaStream_t stream) {
-  return trb_gemm_bf16_ex3(A, lda, a_mn, B, ldb, b_mn, out, ldo, out_f32, M, N, K, bias, act, mask, ld_mask, alpha, split_k, tile_n, mask_bits, relu_bits_out,
-                           ld_bits, nullptr, stream);
-}
-
+// mask_bits / relu_bits_out: int32 [M, ld_bits] bit matrices (bit n % 32 of word n / 32), see GemmParams.
 // colsum_ws: fp32 [ceil(M / 32), N] or nullptr, see GemmParams (bf16 output without split-K only: -14 otherwise).
 // tile_n: tile-width hint of the caller's split-K plan; the tile shape depends on N only (128 x 64, 128 x 128 or 128 x 256).
-TRB_API int trb_gemm_bf16_ex3(const void* A, int64_t lda, int a_mn, const void* B, int64_t ldb, int b_mn, void* out, int64_t ldo, int out_f32, int M,
-                              int N, int K, const float* bias, int act, const void* mask, int64_t ld_mask, float alpha, int split_k, int tile_n,
-                              const void* mask_bits, void* relu_bits_out, int64_t ld_bits, float* colsum_ws, cudaStream_t stream) {
+TRB_API int trb_gemm_bf16(const void* A, int64_t lda, int a_mn, const void* B, int64_t ldb, int b_mn, void* out, int64_t ldo, int out_f32, int M,
+                          int N, int K, const float* bias, int act, const void* mask, int64_t ld_mask, float alpha, int split_k, int tile_n,
+                          const void* mask_bits, void* relu_bits_out, int64_t ld_bits, float* colsum_ws, cudaStream_t stream) {
   if (M <= 0 || N <= 0 || K <= 0) return 0;
   if ((lda % 8) || (ldb % 8) || (N % 8)) return -12;
   if ((!a_mn && (K % 8)) || (a_mn && (M % 8)) || (b_mn && (N % 8)) || (!b_mn && (K % 8))) return -12;
@@ -629,17 +606,6 @@ TRB_API int trb_gemm_bf16_ex3(const void* A, int64_t lda, int a_mn, const void* 
   return gemm_dispatch<false, false>(A, lda, B, ldb, p, stream);
 }
 
-TRB_API int trb_gemm_bf16(const void* A, int64_t lda, int a_mn, const void* B, int64_t ldb, int b_mn, void* out, int64_t ldo, int out_f32, int M,
-                          int N, int K, const float* bias, int act, const void* mask, int64_t ld_mask, float alpha, int split_k,
-                          cudaStream_t stream) {
-  return trb_gemm_bf16_ex(A, lda, a_mn, B, ldb, b_mn, out, ldo, out_f32, M, N, K, bias, act, mask, ld_mask, alpha, split_k, 0, stream);
-}
-
-TRB_API int trb_gemm_bf16_tn(const void* A, int64_t lda, const void* B, int64_t ldb, void* out, int64_t ldo, int out_f32, int M, int N, int K,
-                             const float* bias, int act, const void* mask, int64_t ld_mask, float alpha, int split_k, cudaStream_t stream) {
-  return trb_gemm_bf16(A, lda, 0, B, ldb, 0, out, ldo, out_f32, M, N, K, bias, act, mask, ld_mask, alpha, split_k, stream);
-}
-
 // ---- helpers used around the GEMM ----------------------------------------------------------------------
 // bf16 transpose: out[c, r] = in[r, c]; 32x32 smem tiles, coalesced both ways.
 __global__ void __launch_bounds__(256) trb_transpose_bf16_kernel(const __nv_bfloat16* __restrict__ in, __nv_bfloat16* __restrict__ out, int rows,
@@ -666,49 +632,12 @@ TRB_API int trb_transpose_bf16(const void* in, void* out, int rows, int cols, in
   return 0;
 }
 
-// column sums of a bf16 [rows, cols] matrix into fp32 (bias gradient). Each thread owns 8 columns
-// (one 16 B load per row) and strides over rows; 8 row lanes per block are reduced through smem and
-// the block result is added atomically (blocks tile the rows so the whole chip participates).
-__global__ void __launch_bounds__(256) trb_colsum_bf16_kernel(const __nv_bfloat16* __restrict__ in, float* __restrict__ out, int rows, int cols,
-                                                                int64_t ld, int rows_per_block) {
-  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
-  const int vec = blockIdx.x * 32 + tx;  // 8-column group
-  const int nvec = cols >> 3;
-  const int r0 = blockIdx.y * rows_per_block;
-  const int r1 = min(rows, r0 + rows_per_block);
-  float acc[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) acc[j] = 0.f;
-  if (vec < nvec) {
-    for (int r = r0 + ty; r < r1; r += 8) {
-      const uint4 v = *reinterpret_cast<const uint4*>(in + (int64_t) r * ld + vec * 8);
-      const __nv_bfloat16* b = reinterpret_cast<const __nv_bfloat16*>(&v);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) acc[j] += __bfloat162float(b[j]);
-    }
-  }
-  __shared__ float red[8][32][9];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) red[ty][tx][j] = acc[j];
-  __syncthreads();
-  if (ty == 0 && vec < nvec) {
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      float s = 0.f;
-#pragma unroll
-      for (int i = 0; i < 8; ++i) s += red[i][tx][j];
-      atomicAdd(out + vec * 8 + j, s);
-    }
-  }
-}
-
-// v3: contended fp32 atomics were the bottleneck of v1 (every 128 B line of `out` took rows/256 x 32 serialized L2 atomics).
-// Now: (a) ~4 blocks per SM, each walking a tall row slab with 8 independent 16 B loads in flight per
-// thread, (b) narrow matrices fold several rows into one warp (vpr = lanes per row) so every lane loads, (c) block partials
-// go to a workspace and the LAST block of a column group (ticket counter) sums them in a fixed order: no float atomics,
-// deterministic result, one launch.
+// Column sums of a bf16 [rows, cols] matrix into fp32 (bias gradient): (a) ~4 blocks per SM, each walking a tall row slab with 8
+// independent 16 B loads in flight per thread, (b) narrow matrices fold several rows into one warp (vpr = lanes per row) so every
+// lane loads, (c) block partials go to a workspace and the LAST block of a column group (ticket counter) sums them in a fixed
+// order: no float atomics (contended fp32 atomics on `out` serialise in L2), deterministic result, one launch.
 template <bool CLUSTER>
-__device__ __forceinline__ void colsum_v3_body(const __nv_bfloat16* __restrict__ in, float* __restrict__ out, int rows, int cols, int64_t ld,
+__device__ __forceinline__ void colsum_body(const __nv_bfloat16* __restrict__ in, float* __restrict__ out, int rows, int cols, int64_t ld,
                                                int rows_per_block, int vpr_log2, float* __restrict__ partial, unsigned int* __restrict__ tickets) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int vpr = 1 << vpr_log2, rpw = 32 >> vpr_log2;  // lanes per row, rows per warp
@@ -830,16 +759,16 @@ __device__ __forceinline__ void colsum_v3_body(const __nv_bfloat16* __restrict__
   if (threadIdx.x == 0) tickets[blockIdx.x] = 0;  // ready for the next launch on this stream
 }
 
-__global__ void __launch_bounds__(256) trb_colsum_bf16_v3_kernel(const __nv_bfloat16* __restrict__ in, float* __restrict__ out, int rows, int cols,
+__global__ void __launch_bounds__(256) trb_colsum_bf16_kernel(const __nv_bfloat16* __restrict__ in, float* __restrict__ out, int rows, int cols,
                                                                    int64_t ld, int rows_per_block, int vpr_log2, float* __restrict__ partial,
                                                                    unsigned int* __restrict__ tickets) {
-  colsum_v3_body<false>(in, out, rows, cols, ld, rows_per_block, vpr_log2, partial, tickets);
+  colsum_body<false>(in, out, rows, cols, ld, rows_per_block, vpr_log2, partial, tickets);
 }
 
 __global__ void __cluster_dims__(1, 8, 1) __launch_bounds__(256)
-trb_colsum_bf16_v4_kernel(const __nv_bfloat16* __restrict__ in, float* __restrict__ out, int rows, int cols, int64_t ld, int rows_per_block,
+trb_colsum_bf16_cluster_kernel(const __nv_bfloat16* __restrict__ in, float* __restrict__ out, int rows, int cols, int64_t ld, int rows_per_block,
                           int vpr_log2, float* __restrict__ partial, unsigned int* __restrict__ tickets) {
-  colsum_v3_body<true>(in, out, rows, cols, ld, rows_per_block, vpr_log2, partial, tickets);
+  colsum_body<true>(in, out, rows, cols, ld, rows_per_block, vpr_log2, partial, tickets);
 }
 
 // per-device workspace of the column-sum kernel (tickets + block partials); kernels that use it are stream ordered
@@ -851,53 +780,43 @@ TRB_API int trb_colsum_bf16(const void* in, float* out, int rows, int cols, int6
   if (cols % 8 || ld % 8) return -12;
   const int nvec = cols / 8;
   const int xblocks = (nvec + 31) / 32;
-  static const int variant = [] { const char* e = getenv("TRB_COLSUM"); return e ? atoi(e) : 4; }();
-  if (variant == 3 || variant == 4) {
-    int vpr_log2 = 5;
-    while (vpr_log2 > 0 && (1 << (vpr_log2 - 1)) >= nvec) --vpr_log2;
-    const int rpw = 32 >> vpr_log2;
-    int yblocks = (4 * trb_num_sms() + xblocks - 1) / xblocks;
-    const bool clustered = variant == 4 && rows >= 2048;
-    if (clustered) {
-      if (yblocks > 256) yblocks = 256;  // 8-CTA clusters fold through DSMEM: 32 partials at most reach the last-block tail
-    } else if (yblocks > 64) {
-      yblocks = 64;  // the last block of a column group sums yblocks partials: keep that tail short
-    }
-    int rows_per_block = (rows + yblocks - 1) / yblocks;
-    rows_per_block = (rows_per_block + 8 * rpw - 1) / (8 * rpw) * (8 * rpw);
-    yblocks = (rows + rows_per_block - 1) / rows_per_block;
-    if (clustered) yblocks = (yblocks + 7) / 8 * 8;  // trailing blocks past `rows` contribute zeros
-    // workspace (per process, stream-ordered use: the dense backward runs on one stream): tickets then partial sums
-    const size_t need = 4096 + sizeof(float) * (size_t) yblocks * (size_t) cols;
-    int dev = 0;
-    TRB_CUDA(cudaGetDevice(&dev));
-    if (dev < 0 || dev >= 64) return -12;
-    size_t& g_colsum_ws_bytes = g_colsum_ws_bytes_dev[dev];
-    void*& g_colsum_ws = g_colsum_ws_dev[dev];
-    if (need > g_colsum_ws_bytes) {
-      if (g_colsum_ws) TRB_CUDA(cudaFree(g_colsum_ws));
-      g_colsum_ws_bytes = need < (8u << 20) ? (8u << 20) : need;
-      TRB_CUDA(cudaMalloc(&g_colsum_ws, g_colsum_ws_bytes));
-      TRB_CUDA(cudaMemset(g_colsum_ws, 0, 4096));
-    }
-    if (xblocks > 1024) return -12;
-    dim3 grid(xblocks, yblocks);
-    if (clustered)
-      trb_colsum_bf16_v4_kernel<<<grid, 256, 0, stream>>>((const __nv_bfloat16*) in, out, rows, cols, ld, rows_per_block, vpr_log2,
-                                                          reinterpret_cast<float*>(static_cast<char*>(g_colsum_ws) + 4096),
-                                                          reinterpret_cast<unsigned int*>(g_colsum_ws));
-    else
-      trb_colsum_bf16_v3_kernel<<<grid, 256, 0, stream>>>((const __nv_bfloat16*) in, out, rows, cols, ld, rows_per_block, vpr_log2,
-                                                          reinterpret_cast<float*>(static_cast<char*>(g_colsum_ws) + 4096),
-                                                          reinterpret_cast<unsigned int*>(g_colsum_ws));
-    TRB_CHECK_LAUNCH();
-    return 0;
+  int vpr_log2 = 5;
+  while (vpr_log2 > 0 && (1 << (vpr_log2 - 1)) >= nvec) --vpr_log2;
+  const int rpw = 32 >> vpr_log2;
+  int yblocks = (4 * trb_num_sms() + xblocks - 1) / xblocks;
+  const bool clustered = rows >= 2048;
+  if (clustered) {
+    if (yblocks > 256) yblocks = 256;  // 8-CTA clusters fold through DSMEM: 32 partials at most reach the last-block tail
+  } else if (yblocks > 64) {
+    yblocks = 64;  // the last block of a column group sums yblocks partials: keep that tail short
   }
-  TRB_CUDA(cudaMemsetAsync(out, 0, sizeof(float) * cols, stream));
-  int rows_per_block = 256;
-  while ((int64_t) xblocks * ((rows + rows_per_block - 1) / rows_per_block) > 2048 && rows_per_block < 65536) rows_per_block *= 2;
-  dim3 grid(xblocks, (rows + rows_per_block - 1) / rows_per_block);
-  trb_colsum_bf16_kernel<<<grid, 256, 0, stream>>>((const __nv_bfloat16*) in, out, rows, cols, ld, rows_per_block);
+  int rows_per_block = (rows + yblocks - 1) / yblocks;
+  rows_per_block = (rows_per_block + 8 * rpw - 1) / (8 * rpw) * (8 * rpw);
+  yblocks = (rows + rows_per_block - 1) / rows_per_block;
+  if (clustered) yblocks = (yblocks + 7) / 8 * 8;  // trailing blocks past `rows` contribute zeros
+  // workspace (per process, stream-ordered use: the dense backward runs on one stream): tickets then partial sums
+  const size_t need = 4096 + sizeof(float) * (size_t) yblocks * (size_t) cols;
+  int dev = 0;
+  TRB_CUDA(cudaGetDevice(&dev));
+  if (dev < 0 || dev >= 64) return -12;
+  size_t& g_colsum_ws_bytes = g_colsum_ws_bytes_dev[dev];
+  void*& g_colsum_ws = g_colsum_ws_dev[dev];
+  if (need > g_colsum_ws_bytes) {
+    if (g_colsum_ws) TRB_CUDA(cudaFree(g_colsum_ws));
+    g_colsum_ws_bytes = need < (8u << 20) ? (8u << 20) : need;
+    TRB_CUDA(cudaMalloc(&g_colsum_ws, g_colsum_ws_bytes));
+    TRB_CUDA(cudaMemset(g_colsum_ws, 0, 4096));
+  }
+  if (xblocks > 1024) return -12;
+  dim3 grid(xblocks, yblocks);
+  if (clustered)
+    trb_colsum_bf16_cluster_kernel<<<grid, 256, 0, stream>>>((const __nv_bfloat16*) in, out, rows, cols, ld, rows_per_block, vpr_log2,
+                                                             reinterpret_cast<float*>(static_cast<char*>(g_colsum_ws) + 4096),
+                                                             reinterpret_cast<unsigned int*>(g_colsum_ws));
+  else
+    trb_colsum_bf16_kernel<<<grid, 256, 0, stream>>>((const __nv_bfloat16*) in, out, rows, cols, ld, rows_per_block, vpr_log2,
+                                                     reinterpret_cast<float*>(static_cast<char*>(g_colsum_ws) + 4096),
+                                                     reinterpret_cast<unsigned int*>(g_colsum_ws));
   TRB_CHECK_LAUNCH();
   return 0;
 }

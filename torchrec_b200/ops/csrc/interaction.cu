@@ -15,8 +15,6 @@
 //
 // CTAs are small (128 threads, ~38 KB smem) so several fit per SM and hide the global load latency of
 // each other; each CTA loops over groups of 4 samples.
-#include <cstdlib>
-
 #include "wgmma.cuh"
 
 using namespace trb;
@@ -503,7 +501,7 @@ TRB_API int trb_interaction_fwd(const void* dense, int64_t ld_dense, const void*
   p.out = out; p.ld_out = ld_out; p.B = B; p.F = F; p.out_cols = D + (F + 1) * F / 2;
   if (ld_out % 8 || ld_out < p.out_cols) return -21;
   const int groups = (B + kSamples - 1) / kSamples;
-  if (!sparse_f32 && ld_dense % 8 == 0 && ld_sparse % 8 == 0 && !getenv("TRB_INTERACTION_LEGACY")) {
+  if (!sparse_f32 && ld_dense % 8 == 0 && ld_sparse % 8 == 0) {
     const int smem_p = 4 * kTileBytes + kSamples * (int) ld_out * 2 + 64 + 1024;
     static bool cfg_p = false;
     if (!cfg_p) {
@@ -537,8 +535,7 @@ TRB_API int trb_interaction_bwd(const void* dense, int64_t ld_dense, const void*
   p.gout = gout; p.ld_out = ld_out; p.B = B; p.F = F; p.out_cols = D + (F + 1) * F / 2;
   p.g_dense = g_dense; p.ld_gdense = ld_gdense; p.g_sparse = g_sparse; p.ld_gsparse = ld_gsparse; p.gsparse_f32 = gsparse_f32;
   const int groups = (B + kSamples - 1) / kSamples;
-  if (!sparse_f32 && !gsparse_f32 && ld_dense % 8 == 0 && ld_sparse % 8 == 0 && ld_gdense % 8 == 0 && ld_gsparse % 8 == 0 && ld_out % 8 == 0 &&
-      !getenv("TRB_INTERACTION_LEGACY")) {
+  if (!sparse_f32 && !gsparse_f32 && ld_dense % 8 == 0 && ld_sparse % 8 == 0 && ld_gdense % 8 == 0 && ld_gsparse % 8 == 0 && ld_out % 8 == 0) {
     const int smem_p = 6 * kTileBytes + 2 * kSamples * (int) ld_out * 2 + 64 + 1024;
     static bool cfg_p = false;
     if (!cfg_p) {

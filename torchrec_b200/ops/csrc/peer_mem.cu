@@ -6,7 +6,6 @@
 // load/store them directly over NVSwitch.
 // NCCL stays the control plane (handle exchange, DDP all-reduce, multi-node fallback).
 #include "common.cuh"
-#include <cstdlib>
 #include <cstring>
 #include <cstdio>
 
@@ -297,12 +296,12 @@ TRB_API int trb_grad_push(const void* src, int s_dtype, int64_t src_stride, cons
   for (int i = 0; i < n_dst; ++i) d.p[i] = dst_ptrs[i];
   const int threads = 256;
   constexpr int UNR = 4;
-  static const int ctas_per_sm = getenv("TRB_PUSH_CTAS_PER_SM") ? atoi(getenv("TRB_PUSH_CTAS_PER_SM")) : 2;
+  constexpr int kPushCtasPerSm = 2;  // persistent, but leaves room on every SM for the GEMMs that run beside the push
   int dev = 0, sms = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   int64_t want = (n + (int64_t) threads * UNR - 1) / ((int64_t) threads * UNR);
-  const unsigned blocks = (unsigned) (want < (int64_t) sms * ctas_per_sm ? want : (int64_t) sms * ctas_per_sm);
+  const unsigned blocks = (unsigned) (want < (int64_t) sms * kPushCtasPerSm ? want : (int64_t) sms * kPushCtasPerSm);
 #define TRB_GP(SC, ST, DC, DT)                                                                                                                           \
   if (s_dtype == SC && d_dtype == DC) {                                                                                                                  \
     if (vec == 8) trb_grad_push_kernel<ST, DT, 8, UNR><<<blocks, threads, 0, stream>>>((const ST*) src, src_stride, chunks, n_chunks, d, dst_pitch, row_base, B_local, scale); \

@@ -18,8 +18,6 @@
 // The gradient rows are read through TrbPeerPtrs: with W peer pointers the kernel *pulls*
 // grad[b_local, cols(f)] straight from the rank that owns sample b over NVLink — that is the
 // backward all-to-all of the reference (comm_ops.py:1581-1646) fused into the optimizer kernel.
-#include <cstdlib>
-
 #include "common.cuh"
 #include <cub/device/device_radix_sort.cuh>
 
@@ -73,12 +71,12 @@ struct TbeBwdParams {
   int32_t* bag_of;
   float* partials;  // [chunks][2][max_dim]
   uint8_t* span_flags;
-  uint8_t* chunk_done;  // [chunks] set by tbe_bwd_unique_kernel (nullptr: generic walk handles everything)
+  uint8_t* chunk_done;  // [chunks] set by tbe_bwd_walk_kernel (nullptr: generic walk handles everything)
   int32_t* long_list;   // [chunks] first chunks of spans longer than kLongSpan pieces
   int32_t* long_count;  // zeroed by tbe_bwd_build_keys
   int sr;               // 1: stochastic rounding of the updated row when the table is bf16 / fp16 (unbiased low-precision training)
   unsigned long long sr_seed;
-  int prefetch;         // 1: lanes prefetch their key's rows into L2 ahead of the walk (bit 1: also the gradient rows = local memory)
+  bool prefetch_grad;   // lanes prefetch their key's gradient row into L2 as well as its weight row and row state (gradient in local memory)
   int32_t max_dim;
   int32_t key64;
   int32_t opt;
@@ -176,12 +174,8 @@ __device__ __forceinline__ void trb_store_row4_sr<__half>(__half* dst, float4 v,
 
 // ---- optimizer application on one unique row ------------------------------------------------
 // g[k] holds the summed gradient for elements (lane + 32k)*4 .. +3 of the row.
-// PRE: the caller already issued the loads of the weight row (`wpre`) and, for row-wise Adagrad, of the row state (`spre`, lane 0)
-// BEFORE it accumulated the gradient: the three round trips of a run (gradient rows, weight row, state) overlap instead of
-// following each other.
-template <typename W, int MAXV, bool PRE = false>
-__device__ __forceinline__ void apply_row(const TbeBwdParams& p, int64_t key, int f, float4 (&g)[MAXV], int lane, const float4* wpre = nullptr,
-                                          float spre = 0.f) {
+template <typename W, int MAXV>
+__device__ __forceinline__ void apply_row(const TbeBwdParams& p, int64_t key, int f, float4 (&g)[MAXV], int lane) {
   const int OPT = p.opt;
   const int D = p.feat_dim[f];
   const int nvec = D >> 2;
@@ -195,8 +189,7 @@ __device__ __forceinline__ void apply_row(const TbeBwdParams& p, int64_t key, in
 #pragma unroll
   for (int k = 0; k < MAXV; ++k) {
     const int vi = lane + k * 32;
-    if constexpr (PRE) wv[k] = wpre[k];
-    else wv[k] = (vi < nvec && OPT != OPT_NONE) ? Vec4<W>::ld(w + vi * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
+    wv[k] = (vi < nvec && OPT != OPT_NONE) ? Vec4<W>::ld(w + vi * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
     if (maxg > 0.f) {
       g[k].x = fminf(fmaxf(g[k].x, -maxg), maxg);
       g[k].y = fminf(fmaxf(g[k].y, -maxg), maxg);
@@ -230,7 +223,7 @@ __device__ __forceinline__ void apply_row(const TbeBwdParams& p, int64_t key, in
 #pragma unroll
     for (int k = 0; k < MAXV; ++k) sq += f4_sq(g[k]);  // lanes beyond nvec hold zeros
     sq = warp_sum(sq) / (float) D;
-    float st = PRE ? spre : ((lane == 0) ? p.state1[key] : 0.f);
+    float st = (lane == 0) ? p.state1[key] : 0.f;
     st = __shfl_sync(0xffffffffu, st, 0);
     const float ns = st + sq;
     if (lane == 0) p.state1[key] = ns;
@@ -360,112 +353,6 @@ __device__ __forceinline__ void load_grad_row(const TbeBwdParams& p, int bag, fl
   }
 }
 
-
-// ---- unique-rows kernel ------------------------------------------------------------------------------------------------
-// Handles the chunks whose 32 sorted keys are distinct valid rows that do not continue into the neighbouring chunks (the
-// common case for large tables) when the optimizer is SGD / row-wise Adagrad without clipping or decay; marks them in
-// chunk_done so the generic walk (tbe_bwd_chunk_kernel, lighter on registers, higher occupancy) skips them. Per-lane geometry
-// is computed ONCE in parallel (the generic walk re-derives it per row with integer divisions on every lane) and rows are
-// processed U at a time with all of their gradient / weight / state loads in flight together. The generic path alone was
-// instruction- and latency-bound: one row in flight per warp.
-template <typename W, typename G, int MAXV>
-__global__ void __launch_bounds__(256) tbe_bwd_unique_kernel(const TbeBwdParams p) {
-  typedef uint64_t K;
-  const int lane = threadIdx.x & 31;
-  const int64_t chunk = ((int64_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int64_t base = chunk << 5;
-  if (base >= p.n) return;
-  const int cnt = (int) min((int64_t) 32, p.n - base);
-  const void* keys = p.keys_sorted;
-  const K sentinel = (K) p.total_rows;
-  const K key = lane < cnt ? ld_key(keys, base + lane, p.key64) : sentinel;
-  const bool has_prev = base > 0, has_next = base + 32 < p.n;
-  const K prev_key = has_prev ? ld_key(keys, base - 1, p.key64) : sentinel;
-  const K next_key = has_next ? ld_key(keys, base + 32, p.key64) : sentinel;
-  constexpr int U = MAXV == 1 ? 4 : 2;  // rows in flight per warp (register budget: U x MAXV x 2 float4)
-  const K down = __shfl_down_sync(0xffffffffu, key, 1);
-  const bool lane_ok = lane >= cnt || (key != sentinel && (lane == cnt - 1 || key != down));
-  const K key0 = __shfl_sync(0xffffffffu, key, 0), keyl = __shfl_sync(0xffffffffu, key, cnt - 1);
-  const int OPT = p.opt;
-  if (!__all_sync(0xffffffffu, lane_ok) || (has_prev && prev_key == key0) || (has_next && next_key == keyl) || p.hyper[HP_MAXGRAD] > 0.f) {
-    if (lane == 0) p.chunk_done[chunk] = 0;
-    return;
-  }
-  int bag = 0;
-  float scale = 0.f;
-  if (lane < cnt) {
-    const int val = p.vals_sorted[base + lane];
-    bag = p.bag_of[val];
-    scale = (p.src.psw ? p.src.psw[val] : 1.f) * p.grad_scale;
-    if (p.mean) {
-      const int64_t L = bag_len(p, bag);
-      scale /= (float) (L > 0 ? L : 1);
-    }
-  }
-  int64_t goff = 0, woff = 0;
-  int src_rank = 0, nvec_l = 0;
-  if (lane < cnt) {
-    const int f = bag / p.B;
-    const int b = bag - f * p.B;
-    src_rank = b / p.B_local;
-    const int D = p.feat_dim[f];
-    nvec_l = D >> 2;
-    goff = (int64_t) (b - src_rank * p.B_local) * p.grad_stride + p.feat_col[f];
-    woff = p.feat_woff[f] + ((int64_t) key - p.feat_rowbase[f]) * D;
-  }
-  const float lr = p.hyper[HP_LR], eps = p.hyper[HP_EPS];
-  W* const wbase = reinterpret_cast<W*>(p.weights);
-  for (int j = 0; j < cnt; j += U) {
-    float4 g[U][MAXV], wv[U][MAXV];
-    float st[U];
-    int64_t wo[U], ky[U];
-    int nv[U];
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      const int e = min(j + u, cnt - 1);
-      const int64_t go = __shfl_sync(0xffffffffu, goff, e);
-      wo[u] = __shfl_sync(0xffffffffu, woff, e);
-      ky[u] = (int64_t) __shfl_sync(0xffffffffu, key, e);
-      nv[u] = __shfl_sync(0xffffffffu, nvec_l, e);
-      const float sc = __shfl_sync(0xffffffffu, scale, e);
-      const int sr = __shfl_sync(0xffffffffu, src_rank, e);
-      const G* gp = reinterpret_cast<const G*>(p.grad.p[sr]) + go;
-      const W* wp = wbase + wo[u];
-#pragma unroll
-      for (int k = 0; k < MAXV; ++k) {
-        const int vi = lane + k * 32;
-        g[u][k] = (vi < nv[u]) ? f4_scale(Vec4<G>::ld(gp + vi * 4), sc) : make_float4(0.f, 0.f, 0.f, 0.f);
-        wv[u][k] = (vi < nv[u]) ? Vec4<W>::ld(wp + vi * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-      st[u] = (OPT == OPT_ROWWISE_ADAGRAD) ? p.state1[ky[u]] : 0.f;  // same address on every lane: one broadcast transaction
-    }
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      if (j + u >= cnt) break;
-      float mult = lr;
-      if (OPT == OPT_ROWWISE_ADAGRAD) {
-        float sq = 0.f;
-#pragma unroll
-        for (int k = 0; k < MAXV; ++k) sq += f4_sq(g[u][k]);
-        sq = warp_sum(sq) / (float) (nv[u] << 2);
-        const float ns = st[u] + sq;
-        if (lane == 0) p.state1[ky[u]] = ns;
-        mult = lr / (sqrtf(ns) + eps);
-      }
-      W* wp = wbase + wo[u];
-#pragma unroll
-      for (int k = 0; k < MAXV; ++k) {
-        const int vi = lane + k * 32;
-        if (vi < nv[u]) Vec4<W>::st(wp + vi * 4, f4_fma(g[u][k], -mult, wv[u][k]));
-      }
-    }
-  }
-  if (lane == 0) {
-    p.chunk_done[chunk] = 1;
-    p.span_flags[chunk] = 0;
-  }
-}
-
 // ---- multi-row walk ---------------------------------------------------------------------------------------------------
 // The generic walk below handles one run of equal keys at a time: gradient rows -> weight row -> row state -> store is ONE dependent
 // chain per warp, and every lane re-derives the row geometry (two integer divisions) for every gradient row. For SGD / row-wise Adagrad without clipping
@@ -477,8 +364,12 @@ __global__ void __launch_bounds__(256) tbe_bwd_unique_kernel(const TbeBwdParams 
 //     is warp-uniform. Accumulation order and fma contraction are those of the generic walk: results are bit-identical.
 // Runs that continue into a neighbouring chunk leave partial rows exactly like the generic walk (span kernels combine them).
 // Chunks it handled are marked in chunk_done; the generic kernel returns immediately for those.
-template <typename W, typename G, int MAXV, int MINB, int UU = 0>
-__global__ void __launch_bounds__(256, MINB) tbe_bwd_walk_kernel(const TbeBwdParams p) {
+// Entries in flight per warp vs CTAs per SM (register budget: U x MAXV x 2 float4): D <= 128 (MAXV == 1) walks 2 entries at a time at
+// 4 CTAs per SM, D <= 512 (MAXV == 4) one entry at a time at 3 CTAs per SM.
+template <typename W, typename G, int MAXV>
+__global__ void __launch_bounds__(256, MAXV == 1 ? 4 : 3) tbe_bwd_walk_kernel(const TbeBwdParams p) {
+  static_assert(MAXV == 1 || MAXV == 4, "the walk kernel is built for D <= 128 and D <= 512 only");
+  constexpr int U = MAXV == 1 ? 2 : 1;
   typedef uint64_t K;
   const int lane = threadIdx.x & 31;
   const int64_t chunk = ((int64_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -530,16 +421,15 @@ __global__ void __launch_bounds__(256, MINB) tbe_bwd_walk_kernel(const TbeBwdPar
     goff = (int64_t) (b - src_rank * p.B_local) * p.grad_stride + p.feat_col[f];
     woff = p.feat_woff[f] + ((int64_t) key - p.feat_rowbase[f]) * D;
   }
-  constexpr int U = UU > 0 ? UU : (MAXV == 1 ? 4 : (MAXV == 2 ? 2 : 1));  // entries in flight per warp (register budget: U x MAXV x 2 float4)
   const int OPT = p.opt;
-  if ((p.prefetch & 4) && lane < cnt_v) {
+  if (lane < cnt_v) {
     // every lane pulls the lines of ITS entry (weight row, row state, gradient row) towards L2 now: the U-wide groups below then
     // find them on chip, and the whole chunk (32 rows) is in flight per warp instead of U rows
     const char* pw = reinterpret_cast<const char*>(reinterpret_cast<const W*>(p.weights) + woff);
     const int wbytes = nvec_l * 4 * (int) sizeof(W);
     for (int o = 0; o < wbytes; o += 128) asm volatile("prefetch.global.L2 [%0];" ::"l"(pw + o));
     if (OPT == OPT_ROWWISE_ADAGRAD) asm volatile("prefetch.global.L2 [%0];" ::"l"(p.state1 + key));
-    if (p.prefetch & 2) {
+    if (p.prefetch_grad) {
       const char* pg = reinterpret_cast<const char*>(reinterpret_cast<const G*>(p.grad.p[src_rank]) + goff);
       const int gbytes = nvec_l * 4 * (int) sizeof(G);
       for (int o = 0; o < gbytes; o += 128) asm volatile("prefetch.global.L2 [%0];" ::"l"(pg + o));
@@ -555,7 +445,6 @@ __global__ void __launch_bounds__(256, MINB) tbe_bwd_walk_kernel(const TbeBwdPar
     typename Vec4<G>::raw g[U][MAXV];  // raw registers: converted when consumed, so all loads of the group are issued first
     typename Vec4<W>::raw wv[U][MAXV];
     float st[U], sc[U];
-    int64_t wo[U], ky[U];
     int nv[U];
 #pragma unroll
     for (int u = 0; u < U; ++u) {
@@ -572,19 +461,16 @@ __global__ void __launch_bounds__(256, MINB) tbe_bwd_walk_kernel(const TbeBwdPar
         g[u][k] = Vec4<G>::ld_raw(gp + ((vi < nv[u]) ? vi * 4 : 0));
       }
       const bool fin = j + u < cnt_v && ((ends >> e) & 1u) && !(head_open && e == e_first_end) && !(tail_open && e == cnt_v - 1);
-      wo[u] = 0;
-      ky[u] = 0;
-      st[u] = 0.f;
-      if (fin) {  // this entry closes a run that lives entirely inside the chunk: fetch its row now, consume it below
-        wo[u] = __shfl_sync(0xffffffffu, woff, e);
-        ky[u] = (int64_t) __shfl_sync(0xffffffffu, key, e);
-        const W* wp = wbase + wo[u];
+      // this entry closes a run that lives entirely inside the chunk: fetch its row now, consume it below (wv / st are read for
+      // such entries only; their weight offset and key are shuffled again where they are stored, instead of staying live in registers)
+      if (fin) {
+        const W* wp = wbase + __shfl_sync(0xffffffffu, woff, e);
 #pragma unroll
         for (int k = 0; k < MAXV; ++k) {
           const int vi = lane + k * 32;
           wv[u][k] = Vec4<W>::ld_raw(wp + ((vi < nv[u]) ? vi * 4 : 0));
         }
-        if (OPT == OPT_ROWWISE_ADAGRAD && !(p.prefetch & 8)) st[u] = p.state1[ky[u]];  // same address on every lane: one broadcast transaction
+        if (OPT == OPT_ROWWISE_ADAGRAD) st[u] = p.state1[__shfl_sync(0xffffffffu, key, e)];  // same address on every lane: one broadcast transaction
       }
     }
     // Group of U DISTINCT rows that all live inside the chunk (the common case for large tables): the U updates are independent, so
@@ -616,7 +502,8 @@ __global__ void __launch_bounds__(256, MINB) tbe_bwd_walk_kernel(const TbeBwdPar
 #pragma unroll
           for (int u = 0; u < U; ++u) {
             const float ns = st[u] + sq[u] / (float) (nv[u] << 2);
-            if (lane == 0 && !(p.prefetch & 8)) p.state1[ky[u]] = ns;
+            const K k_u = __shfl_sync(0xffffffffu, key, j + u);
+            if (lane == 0) p.state1[k_u] = ns;
             mult[u] = lr / (sqrtf(ns) + eps);
           }
         } else {
@@ -625,7 +512,7 @@ __global__ void __launch_bounds__(256, MINB) tbe_bwd_walk_kernel(const TbeBwdPar
         }
 #pragma unroll
         for (int u = 0; u < U; ++u) {
-          W* wp = wbase + wo[u];
+          W* wp = wbase + __shfl_sync(0xffffffffu, woff, j + u);
 #pragma unroll
           for (int k = 0; k < MAXV; ++k) {
             const int vi = lane + k * 32;
@@ -652,10 +539,11 @@ __global__ void __launch_bounds__(256, MINB) tbe_bwd_walk_kernel(const TbeBwdPar
           for (int k = 0; k < MAXV; ++k) sq += f4_sq(acc[k]);
           sq = warp_sum(sq) / (float) (nv[u] << 2);
           const float ns = st[u] + sq;
-          if (lane == 0 && !(p.prefetch & 8)) p.state1[ky[u]] = ns;
+          const K k_u = __shfl_sync(0xffffffffu, key, e);
+          if (lane == 0) p.state1[k_u] = ns;
           mult = lr / (sqrtf(ns) + eps);
         }
-        W* wp = wbase + wo[u];
+        W* wp = wbase + __shfl_sync(0xffffffffu, woff, e);
 #pragma unroll
         for (int k = 0; k < MAXV; ++k) {
           const int vi = lane + k * 32;
@@ -688,7 +576,7 @@ __global__ void __launch_bounds__(256) tbe_bwd_chunk_kernel(const TbeBwdParams p
   const int64_t chunk = ((int64_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int64_t base = chunk << 5;
   if (base >= p.n) return;
-  if (p.chunk_done != nullptr && p.chunk_done[chunk]) return;  // already handled by tbe_bwd_walk_kernel / tbe_bwd_unique_kernel
+  if (p.chunk_done != nullptr && p.chunk_done[chunk]) return;  // already handled by tbe_bwd_walk_kernel
   const int cnt = (int) min((int64_t) 32, p.n - base);
   const void* keys = p.keys_sorted;
   const K sentinel = (K) p.total_rows;
@@ -719,7 +607,7 @@ __global__ void __launch_bounds__(256) tbe_bwd_chunk_kernel(const TbeBwdParams p
   const char* pf_g = nullptr;
   const char* pf_s = nullptr;
   int pf_wbytes = 0, pf_gbytes = 0;
-  if (p.prefetch && lane < cnt && key != sentinel) {
+  if (lane < cnt && key != sentinel) {
     const int pf = bag / p.B;
     const int pb = bag - pf * p.B;
     const int ps = pb / p.B_local;
@@ -727,7 +615,7 @@ __global__ void __launch_bounds__(256) tbe_bwd_chunk_kernel(const TbeBwdParams p
     pf_w = reinterpret_cast<const char*>(reinterpret_cast<const W*>(p.weights) + p.feat_woff[pf] + ((int64_t) key - p.feat_rowbase[pf]) * pD);
     pf_wbytes = p.opt == OPT_NONE ? 0 : pD * (int) sizeof(W);
     pf_g = reinterpret_cast<const char*>(reinterpret_cast<const G*>(p.grad.p[ps]) + (int64_t) (pb - ps * p.B_local) * p.grad_stride + p.feat_col[pf]);
-    pf_gbytes = (p.prefetch & 2) ? pD * (int) sizeof(G) : 0;
+    pf_gbytes = p.prefetch_grad ? pD * (int) sizeof(G) : 0;
     if (p.opt == OPT_ROWWISE_ADAGRAD) pf_s = reinterpret_cast<const char*>(p.state1 + key);
   }
   auto prefetch_mine = [&]() {
@@ -989,24 +877,12 @@ static int run_bwd(TbeBwdParams& p, char* ws, cudaStream_t stream) {
   if (p.phase == 1) return 0;
   const int64_t chunks = (p.n + 31) / 32;
   const int64_t blocks = (chunks + 7) / 8;
-  // pass 1 (optional): chunks of distinct rows with a simple optimizer go through the high-MLP unique kernel
-  static const int fast_enabled = getenv("TRB_BWD_UNIQUE") ? atoi(getenv("TRB_BWD_UNIQUE")) : 0;  // opt-in
-  static const int walk_enabled = getenv("TRB_BWD_WALK") ? atoi(getenv("TRB_BWD_WALK")) : 1;
+  // pass 1: SGD / row-wise Adagrad without weight decay or stochastic rounding walk their chunks several entries at a time
   const bool simple_opt = (p.opt == OPT_SGD || p.opt == OPT_ROWWISE_ADAGRAD) && p.wd_mode == 0 && !(sizeof(W) == 2 && p.sr);
   if constexpr (MAXV <= 4) {
-    if (walk_enabled && simple_opt) {
+    if (simple_opt) {
       p.chunk_done = (uint8_t*) (ws + L.done);
-      // entries in flight per warp vs CTAs per SM. One H100, 4 tables x 262144 distinct ids (tools/kernel_bench.py): =1 775 us,
-      // =2 732 us, =3 814 us; =1 stays the default until the choice is re-measured on the whole step.
-      // TRB_BWD_WALK=1 (default): D <= 128 -> 2 entries / 4 CTAs per SM; =3: 4 entries / 3 CTAs; =2: 4 entries / 2 CTAs
-      if (walk_enabled == 2) tbe_bwd_walk_kernel<W, G, MAXV, 2><<<(unsigned) blocks, threads, 0, stream>>>(p);
-      else if (walk_enabled == 3 && MAXV == 1) tbe_bwd_walk_kernel<W, G, MAXV, 3, 4><<<(unsigned) blocks, threads, 0, stream>>>(p);   // 4 entries in flight, 3 CTAs / SM
-      else if (MAXV == 1) tbe_bwd_walk_kernel<W, G, MAXV, 4, 2><<<(unsigned) blocks, threads, 0, stream>>>(p);   // default: 2 entries in flight, 4 CTAs / SM
-      else tbe_bwd_walk_kernel<W, G, MAXV, 3><<<(unsigned) blocks, threads, 0, stream>>>(p);
-      TRB_CHECK_LAUNCH();
-    } else if (fast_enabled && simple_opt) {
-      p.chunk_done = (uint8_t*) (ws + L.done);
-      tbe_bwd_unique_kernel<W, G, MAXV><<<(unsigned) blocks, threads, 0, stream>>>(p);
+      tbe_bwd_walk_kernel<W, G, MAXV><<<(unsigned) blocks, threads, 0, stream>>>(p);
       TRB_CHECK_LAUNCH();
     }
   }
@@ -1033,40 +909,18 @@ static int dispatch_dim(TbeBwdParams& p, char* ws, cudaStream_t stream) {
   return -2;
 }
 
-TRB_API int trb_tbe_bwd_fused_phase(void* weights, int w_dtype, float* state1, float* state2, const float* hyper, int opt,
-                                    int wd_mode, const int64_t* feat_woff, const int64_t* feat_rows,
-                                    const int64_t* feat_rowbase, const int32_t* feat_dim, const int32_t* feat_col,
-                                    const void* indices, int idx64, const void* offsets, int off64, const float* psw,
-                                    int n_src, int64_t idx_stride, int64_t off_stride,
-                                    void* const* grad_ptrs, int n_grad, int grad_dtype, int64_t grad_stride, float grad_scale, int64_t n,
-                                    int64_t total_rows, int B, int B_local, int F, int max_dim, int mean, void* workspace,
-                                    int stochastic_rounding, unsigned long long sr_seed, int phase, cudaStream_t stream);
-
 // Fused backward + optimizer. `workspace` must hold trb_tbe_bwd_workspace_bytes(n, max_dim, total_rows).
 // `n` = number of id POSITIONS to scan (capacity of `indices`; with n_src > 1 it must equal n_src * idx_stride).
-TRB_API int trb_tbe_bwd_fused_ms(void* weights, int w_dtype, float* state1, float* state2, const float* hyper, int opt,
-                                 int wd_mode, const int64_t* feat_woff, const int64_t* feat_rows,
-                                 const int64_t* feat_rowbase, const int32_t* feat_dim, const int32_t* feat_col,
-                                 const void* indices, int idx64, const void* offsets, int off64, const float* psw,
-                                 int n_src, int64_t idx_stride, int64_t off_stride,
-                                 void* const* grad_ptrs, int n_grad, int grad_dtype, int64_t grad_stride, float grad_scale, int64_t n,
-                                 int64_t total_rows, int B, int B_local, int F, int max_dim, int mean, void* workspace,
-                                 int stochastic_rounding, unsigned long long sr_seed, cudaStream_t stream) {
-  return trb_tbe_bwd_fused_phase(weights, w_dtype, state1, state2, hyper, opt, wd_mode, feat_woff, feat_rows, feat_rowbase, feat_dim, feat_col, indices, idx64,
-                                 offsets, off64, psw, n_src, idx_stride, off_stride, grad_ptrs, n_grad, grad_dtype, grad_stride, grad_scale, n, total_rows, B,
-                                 B_local, F, max_dim, mean, workspace, stochastic_rounding, sr_seed, 0, stream);
-}
-
 // phase 1 = prepare (keys + radix sort; needs only the ids: run it as soon as the ids exist, off the critical path);
 // phase 2 = apply (run walk + optimizer; needs the gradient and the workspace filled by phase 1); phase 0 = both.
-TRB_API int trb_tbe_bwd_fused_phase(void* weights, int w_dtype, float* state1, float* state2, const float* hyper, int opt,
-                                    int wd_mode, const int64_t* feat_woff, const int64_t* feat_rows,
-                                    const int64_t* feat_rowbase, const int32_t* feat_dim, const int32_t* feat_col,
-                                    const void* indices, int idx64, const void* offsets, int off64, const float* psw,
-                                    int n_src, int64_t idx_stride, int64_t off_stride,
-                                    void* const* grad_ptrs, int n_grad, int grad_dtype, int64_t grad_stride, float grad_scale, int64_t n,
-                                    int64_t total_rows, int B, int B_local, int F, int max_dim, int mean, void* workspace,
-                                    int stochastic_rounding, unsigned long long sr_seed, int phase, cudaStream_t stream) {
+TRB_API int trb_tbe_bwd_fused(void* weights, int w_dtype, float* state1, float* state2, const float* hyper, int opt,
+                              int wd_mode, const int64_t* feat_woff, const int64_t* feat_rows,
+                              const int64_t* feat_rowbase, const int32_t* feat_dim, const int32_t* feat_col,
+                              const void* indices, int idx64, const void* offsets, int off64, const float* psw,
+                              int n_src, int64_t idx_stride, int64_t off_stride,
+                              void* const* grad_ptrs, int n_grad, int grad_dtype, int64_t grad_stride, float grad_scale, int64_t n,
+                              int64_t total_rows, int B, int B_local, int F, int max_dim, int mean, void* workspace,
+                              int stochastic_rounding, unsigned long long sr_seed, int phase, cudaStream_t stream) {
   if (n <= 0) return 0;
   if (n_grad < 1 || n_grad > TRB_MAX_PEERS) return -1;
   if ((int64_t) B_local * n_grad != B) return -4;
@@ -1108,14 +962,7 @@ TRB_API int trb_tbe_bwd_fused_phase(void* weights, int w_dtype, float* state1, f
   p.opt = opt;
   p.sr = stochastic_rounding ? 1 : 0;
   p.sr_seed = sr_seed;
-  {
-    static const int pf = getenv("TRB_BWD_PREFETCH") ? atoi(getenv("TRB_BWD_PREFETCH")) : 1;
-    static const int wpf = getenv("TRB_BWD_WALK_PF") ? atoi(getenv("TRB_BWD_WALK_PF")) : 1;
-    p.prefetch = pf ? (1 | (n_grad <= 1 ? 2 : 0)) : 0;  // peer-resident gradient rows bypass the local L2: do not prefetch them
-    if (wpf) p.prefetch |= 4 | (wpf >= 2 && n_grad <= 1 ? 2 : 0);
-    static const int nostate = getenv("TRB_BWD_DEBUG_NOSTATE") ? atoi(getenv("TRB_BWD_DEBUG_NOSTATE")) : 0;  // measurement aid: skip the row-state memory traffic
-    if (nostate) p.prefetch |= 8;
-  }
+  p.prefetch_grad = n_grad <= 1;  // peer-resident gradient rows bypass the local L2: do not prefetch them
   if (opt < 0 || opt > OPT_LION) return -5;
   char* ws = reinterpret_cast<char*>(workspace);
 #define TRB_BWD_CASE(WC, WT, GC, GT) \
@@ -1127,28 +974,4 @@ TRB_API int trb_tbe_bwd_fused_phase(void* weights, int w_dtype, float* state1, f
   TRB_BWD_CASE(TRB_F16, __half, TRB_F32, float);
 #undef TRB_BWD_CASE
   return -3;
-}
-
-TRB_API int trb_tbe_bwd_fused_ex(void* weights, int w_dtype, float* state1, float* state2, const float* hyper, int opt,
-                                 int wd_mode, const int64_t* feat_woff, const int64_t* feat_rows,
-                                 const int64_t* feat_rowbase, const int32_t* feat_dim, const int32_t* feat_col,
-                                 const void* indices, int idx64, const void* offsets, int off64, const float* psw,
-                                 void* const* grad_ptrs, int n_grad, int grad_dtype, int64_t grad_stride, int64_t n,
-                                 int64_t total_rows, int B, int B_local, int F, int max_dim, int mean, void* workspace,
-                                 int stochastic_rounding, unsigned long long sr_seed, cudaStream_t stream) {
-  return trb_tbe_bwd_fused_ms(weights, w_dtype, state1, state2, hyper, opt, wd_mode, feat_woff, feat_rows, feat_rowbase, feat_dim, feat_col, indices,
-                              idx64, offsets, off64, psw, 1, 0, 0, grad_ptrs, n_grad, grad_dtype, grad_stride, 1.f, n, total_rows, B, B_local, F,
-                              max_dim, mean, workspace, stochastic_rounding, sr_seed, stream);
-}
-
-TRB_API int trb_tbe_bwd_fused(void* weights, int w_dtype, float* state1, float* state2, const float* hyper, int opt,
-                              int wd_mode, const int64_t* feat_woff, const int64_t* feat_rows,
-                              const int64_t* feat_rowbase, const int32_t* feat_dim, const int32_t* feat_col,
-                              const void* indices, int idx64, const void* offsets, int off64, const float* psw,
-                              void* const* grad_ptrs, int n_grad, int grad_dtype, int64_t grad_stride, int64_t n,
-                              int64_t total_rows, int B, int B_local, int F, int max_dim, int mean, void* workspace,
-                              cudaStream_t stream) {
-  return trb_tbe_bwd_fused_ex(weights, w_dtype, state1, state2, hyper, opt, wd_mode, feat_woff, feat_rows, feat_rowbase, feat_dim, feat_col, indices,
-                              idx64, offsets, off64, psw, grad_ptrs, n_grad, grad_dtype, grad_stride, n, total_rows, B, B_local, F, max_dim, mean,
-                              workspace, 0, 0ull, stream);
 }

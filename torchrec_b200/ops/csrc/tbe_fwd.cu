@@ -314,11 +314,11 @@ static int dispatch_out(const TbeFwdParams& p, int out_dtype, int max_dim, cudaS
 
 // Pooled forward. Returns 0 on success, a cudaError_t (>0) or a negative library error.
 // `n_src` > 1: ids arrive in per-source regions (see TrbSrcView); idx_stride / off_stride in elements.
-TRB_API int trb_tbe_pooled_fwd_ms(const void* weights, int w_dtype, const int64_t* feat_woff, const int64_t* feat_rows,
-                                  const int32_t* feat_dim, const int32_t* feat_col, const void* indices, int idx64,
-                                  const void* offsets, int off64, const float* psw, int n_src, int64_t idx_stride, int64_t off_stride,
-                                  void* const* out_ptrs, int n_out, int out_dtype, int64_t out_stride, int B, int B_local, int F,
-                                  int max_dim, int mean, cudaStream_t stream) {
+TRB_API int trb_tbe_pooled_fwd(const void* weights, int w_dtype, const int64_t* feat_woff, const int64_t* feat_rows,
+                               const int32_t* feat_dim, const int32_t* feat_col, const void* indices, int idx64,
+                               const void* offsets, int off64, const float* psw, int n_src, int64_t idx_stride, int64_t off_stride,
+                               void* const* out_ptrs, int n_out, int out_dtype, int64_t out_stride, int B, int B_local, int F,
+                               int max_dim, int mean, cudaStream_t stream) {
   if (n_out < 1 || n_out > TRB_MAX_PEERS) return -1;
   if ((int64_t) B_local * n_out != B) return -4;
   if (n_src < 1 || B % n_src != 0) return -4;
@@ -350,15 +350,6 @@ TRB_API int trb_tbe_pooled_fwd_ms(const void* weights, int w_dtype, const int64_
     case TRB_BF16: return dispatch_out<__nv_bfloat16>(p, out_dtype, max_dim, stream);
   }
   return -3;
-}
-
-TRB_API int trb_tbe_pooled_fwd(const void* weights, int w_dtype, const int64_t* feat_woff, const int64_t* feat_rows,
-                               const int32_t* feat_dim, const int32_t* feat_col, const void* indices, int idx64,
-                               const void* offsets, int off64, const float* psw, void* const* out_ptrs, int n_out,
-                               int out_dtype, int64_t out_stride, int B, int B_local, int F, int max_dim, int mean,
-                               cudaStream_t stream) {
-  return trb_tbe_pooled_fwd_ms(weights, w_dtype, feat_woff, feat_rows, feat_dim, feat_col, indices, idx64, offsets, off64, psw, 1, 0, 0,
-                               out_ptrs, n_out, out_dtype, out_stride, B, B_local, F, max_dim, mean, stream);
 }
 
 // ------------------------------------------------------------------------------------------

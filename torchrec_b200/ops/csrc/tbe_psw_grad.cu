@@ -79,10 +79,10 @@ static int launch_psw(const PswGradParams& p, int max_dim, cudaStream_t stream) 
   return 0;
 }
 
-TRB_API int trb_tbe_psw_grad_ms(const void* weights, int w_dtype, const int64_t* feat_woff, const int64_t* feat_rows, const int32_t* feat_dim,
-                                const int32_t* feat_col, const void* indices, int idx64, const void* offsets, int off64, int n_src, int64_t idx_stride,
-                                int64_t off_stride, void* const* grad_ptrs, int n_grad, int grad_dtype, int64_t grad_stride, float* out, int B,
-                                int B_local, int F, int max_dim, int mean, cudaStream_t stream) {
+TRB_API int trb_tbe_psw_grad(const void* weights, int w_dtype, const int64_t* feat_woff, const int64_t* feat_rows, const int32_t* feat_dim,
+                             const int32_t* feat_col, const void* indices, int idx64, const void* offsets, int off64, int n_src, int64_t idx_stride,
+                             int64_t off_stride, void* const* grad_ptrs, int n_grad, int grad_dtype, int64_t grad_stride, float* out, int B,
+                             int B_local, int F, int max_dim, int mean, cudaStream_t stream) {
   if (n_grad < 1 || n_grad > TRB_MAX_PEERS) return -1;
   if (n_src < 1 || B % n_src != 0) return -4;
   PswGradParams p;
@@ -101,12 +101,4 @@ TRB_API int trb_tbe_psw_grad_ms(const void* weights, int w_dtype, const int64_t*
   PSW_CASE(TRB_F16, __half, TRB_F32, float)
 #undef PSW_CASE
   return -3;
-}
-
-TRB_API int trb_tbe_psw_grad(const void* weights, int w_dtype, const int64_t* feat_woff, const int64_t* feat_rows, const int32_t* feat_dim,
-                             const int32_t* feat_col, const void* indices, int idx64, const void* offsets, int off64, void* const* grad_ptrs,
-                             int n_grad, int grad_dtype, int64_t grad_stride, float* out, int B, int B_local, int F, int max_dim, int mean,
-                             cudaStream_t stream) {
-  return trb_tbe_psw_grad_ms(weights, w_dtype, feat_woff, feat_rows, feat_dim, feat_col, indices, idx64, offsets, off64, 1, 0, 0, grad_ptrs, n_grad,
-                             grad_dtype, grad_stride, out, B, B_local, F, max_dim, mean, stream);
 }

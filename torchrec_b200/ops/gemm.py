@@ -67,14 +67,14 @@ def gemm_bf16(a: torch.Tensor, b: torch.Tensor, a_mn: bool = False, b_mn: bool =
     if colsum_ws is not None:  # fp32 [ceil(M / 32), N]: per-32-row column sums of the bf16 output, written by the epilogue
         assert colsum_ws.dtype == torch.float32 and colsum_ws.is_contiguous() and tuple(colsum_ws.shape) == ((M + 31) // 32, N) and out.dtype == torch.bfloat16 and split_k <= 1
     L = _lib.lib()
-    code = L.trb_gemm_bf16_ex3(
+    code = L.trb_gemm_bf16(
         _lib.ptr(a), ctypes.c_int64(a.stride(0)), int(a_mn), _lib.ptr(b), ctypes.c_int64(b.stride(0)), int(b_mn), _lib.ptr(out),
         ctypes.c_int64(out.stride(0)), 1 if out.dtype == torch.float32 else 0, M, N, K, _lib.ptr(bias), act, _lib.ptr(mask),
         ctypes.c_int64(mask.stride(0) if mask is not None else 0), ctypes.c_float(alpha), int(split_k), int(tile_n),
         _lib.ptr(mask_bits if act == ACT_RELU_GRAD else None), _lib.ptr(relu_bits_out if act == ACT_RELU else None), ctypes.c_int64(ld_bits),
         _lib.ptr(colsum_ws), _lib.stream_ptr(a.device),
     )
-    _lib.check(code, "trb_gemm_bf16_ex3")
+    _lib.check(code, "trb_gemm_bf16")
     return out
 
 

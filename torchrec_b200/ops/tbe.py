@@ -411,7 +411,7 @@ def pooled_forward(
         _lib.ptr(weights), _lib.dtype_code(weights.dtype),
         _lib.ptr(meta.feat_woff), _lib.ptr(meta.feat_rows), _lib.ptr(meta.feat_dim), _lib.ptr(meta.feat_col),
         _lib.ptr(indices), _is64(indices), _lib.ptr(offsets), _is64(offsets),
-        _lib.ptr(per_sample_weights), _lib.ptr_array(out_ptrs), len(out_ptrs),
+        _lib.ptr(per_sample_weights), 1, ctypes.c_int64(0), ctypes.c_int64(0), _lib.ptr_array(out_ptrs), len(out_ptrs),
         _lib.dtype_code(out_dtype), ctypes.c_int64(out_stride), B, B_local, meta.num_features,
         meta.max_dim, int(mean), _lib.stream_ptr(indices.device),
     )
@@ -498,16 +498,16 @@ def fused_backward(
     L.trb_tbe_bwd_workspace_bytes.restype = ctypes.c_int64
     nbytes = L.trb_tbe_bwd_workspace_bytes(ctypes.c_int64(n), meta.max_dim, ctypes.c_int64(meta.total_rows))
     ws = _workspace(nbytes, indices.device)
-    code = L.trb_tbe_bwd_fused_ex(
+    code = L.trb_tbe_bwd_fused(
         _lib.ptr(weights), _lib.dtype_code(weights.dtype), _lib.ptr(state1), _lib.ptr(state2), _lib.ptr(hyper_dev),
         opt, wd_mode, _lib.ptr(meta.feat_woff), _lib.ptr(meta.feat_rows), _lib.ptr(meta.feat_rowbase),
         _lib.ptr(meta.feat_dim), _lib.ptr(meta.feat_col), _lib.ptr(indices), _is64(indices), _lib.ptr(offsets),
-        _is64(offsets), _lib.ptr(per_sample_weights), _lib.ptr_array(grad_ptrs), len(grad_ptrs),
-        _lib.dtype_code(grad_dtype), ctypes.c_int64(grad_stride), ctypes.c_int64(n), ctypes.c_int64(meta.total_rows),
+        _is64(offsets), _lib.ptr(per_sample_weights), 1, ctypes.c_int64(0), ctypes.c_int64(0), _lib.ptr_array(grad_ptrs), len(grad_ptrs),
+        _lib.dtype_code(grad_dtype), ctypes.c_int64(grad_stride), ctypes.c_float(1.0), ctypes.c_int64(n), ctypes.c_int64(meta.total_rows),
         B, B_local, meta.num_features, meta.max_dim, int(mean), _lib.ptr(ws), int(bool(stochastic_rounding)), ctypes.c_uint64(int(sr_seed) & 0xFFFFFFFFFFFFFFFF),
-        _lib.stream_ptr(indices.device),
+        0, _lib.stream_ptr(indices.device),
     )
-    _lib.check(code, "trb_tbe_bwd_fused_ex")
+    _lib.check(code, "trb_tbe_bwd_fused")
 
 
 @dataclass
@@ -541,12 +541,12 @@ def pooled_forward_regions(meta: TbeMeta, weights: torch.Tensor, ids: IdRegions,
     """Pooled lookup over per-source id regions, pooled rows stored into ``out_ptrs`` (one buffer per destination rank)."""
     L = _lib.lib()
     B = ids.n_src * ids.src_B
-    code = L.trb_tbe_pooled_fwd_ms(
+    code = L.trb_tbe_pooled_fwd(
         _lib.ptr(weights), _lib.dtype_code(weights.dtype), _lib.ptr(meta.feat_woff), _lib.ptr(meta.feat_rows), _lib.ptr(meta.feat_dim), _lib.ptr(meta.feat_col),
         ctypes.c_void_p(ids.idx_ptr), ids.idx64, ctypes.c_void_p(ids.off_ptr), ids.off64, ctypes.c_void_p(ids.psw_ptr), ids.n_src,
         ctypes.c_int64(ids.idx_stride), ctypes.c_int64(ids.off_stride), _lib.ptr_array(out_ptrs), len(out_ptrs), _lib.dtype_code(out_dtype),
         ctypes.c_int64(out_stride), B, B_local, meta.num_features, meta.max_dim, int(mean), _lib.stream_ptr(device))
-    _lib.check(code, "trb_tbe_pooled_fwd_ms")
+    _lib.check(code, "trb_tbe_pooled_fwd")
 
 
 def backward_workspace_bytes(n_positions: int, max_dim: int, total_rows: int) -> int:
@@ -563,7 +563,7 @@ def fused_backward_regions(meta: TbeMeta, weights: torch.Tensor, state1, state2,
     any stream; ``phase`` 2 runs the gradient-dependent half (run walk + optimizer) over a prepared workspace; 0 = both."""
     L = _lib.lib()
     B = ids.n_src * ids.src_B
-    code = L.trb_tbe_bwd_fused_phase(
+    code = L.trb_tbe_bwd_fused(
         _lib.ptr(weights), _lib.dtype_code(weights.dtype), _lib.ptr(state1), _lib.ptr(state2), _lib.ptr(hyper_dev), opt, wd_mode,
         _lib.ptr(meta.feat_woff), _lib.ptr(meta.feat_rows), _lib.ptr(meta.feat_rowbase), _lib.ptr(meta.feat_dim), _lib.ptr(meta.feat_col),
         ctypes.c_void_p(ids.idx_ptr), ids.idx64, ctypes.c_void_p(ids.off_ptr), ids.off64, ctypes.c_void_p(ids.psw_ptr), ids.n_src,
@@ -571,7 +571,7 @@ def fused_backward_regions(meta: TbeMeta, weights: torch.Tensor, state1, state2,
         ctypes.c_int64(grad_stride), ctypes.c_float(grad_scale), ctypes.c_int64(ids.positions), ctypes.c_int64(meta.total_rows), B, B_local,
         meta.num_features, meta.max_dim, int(mean), _lib.ptr(workspace), int(bool(stochastic_rounding)), ctypes.c_uint64(int(sr_seed) & 0xFFFFFFFFFFFFFFFF),
         int(phase), _lib.stream_ptr(device))
-    _lib.check(code, "trb_tbe_bwd_fused_phase")
+    _lib.check(code, "trb_tbe_bwd_fused")
 
 
 def psw_grad_regions(meta: TbeMeta, weights: torch.Tensor, ids: IdRegions, mean: bool, grad_ptrs: Sequence[int], grad_stride: int, grad_dtype: torch.dtype,
@@ -579,12 +579,12 @@ def psw_grad_regions(meta: TbeMeta, weights: torch.Tensor, ids: IdRegions, mean:
     """Per-sample-weight gradient over per-source id regions; ``out`` is fp32 ``[positions]`` (position = s * idx_stride + i)."""
     L = _lib.lib()
     B = ids.n_src * ids.src_B
-    code = L.trb_tbe_psw_grad_ms(
+    code = L.trb_tbe_psw_grad(
         _lib.ptr(weights), _lib.dtype_code(weights.dtype), _lib.ptr(meta.feat_woff), _lib.ptr(meta.feat_rows), _lib.ptr(meta.feat_dim), _lib.ptr(meta.feat_col),
         ctypes.c_void_p(ids.idx_ptr), ids.idx64, ctypes.c_void_p(ids.off_ptr), ids.off64, ids.n_src, ctypes.c_int64(ids.idx_stride),
         ctypes.c_int64(ids.off_stride), _lib.ptr_array(grad_ptrs), len(grad_ptrs), _lib.dtype_code(grad_dtype), ctypes.c_int64(grad_stride), _lib.ptr(out),
         B, B_local, meta.num_features, meta.max_dim, int(mean), _lib.stream_ptr(out.device))
-    _lib.check(code, "trb_tbe_psw_grad_ms")
+    _lib.check(code, "trb_tbe_psw_grad")
     return out
 
 
@@ -624,8 +624,8 @@ def psw_grad(meta: TbeMeta, weights: torch.Tensor, indices: torch.Tensor, offset
         grad_ptrs, grad_stride, grad_dtype, B_local = [grad.data_ptr()], grad.stride(0), grad.dtype, B
     L = _lib.lib()
     code = L.trb_tbe_psw_grad(_lib.ptr(weights), _lib.dtype_code(weights.dtype), _lib.ptr(meta.feat_woff), _lib.ptr(meta.feat_rows), _lib.ptr(meta.feat_dim),
-                              _lib.ptr(meta.feat_col), _lib.ptr(indices), _is64(indices), _lib.ptr(offsets), _is64(offsets), _lib.ptr_array(grad_ptrs),
-                              len(grad_ptrs), _lib.dtype_code(grad_dtype), ctypes.c_int64(grad_stride), _lib.ptr(out), B, B_local, meta.num_features,
+                              _lib.ptr(meta.feat_col), _lib.ptr(indices), _is64(indices), _lib.ptr(offsets), _is64(offsets), 1, ctypes.c_int64(0),
+                              ctypes.c_int64(0), _lib.ptr_array(grad_ptrs), len(grad_ptrs), _lib.dtype_code(grad_dtype), ctypes.c_int64(grad_stride), _lib.ptr(out), B, B_local, meta.num_features,
                               meta.max_dim, int(mean), _lib.stream_ptr(indices.device))
     _lib.check(code, "trb_tbe_psw_grad")
     return out

@@ -361,7 +361,9 @@ __device__ __forceinline__ void load_grad_row(const TbeBwdParams& p, int bag, fl
 //   * the U gradient rows AND the weight rows / row states of the runs that end inside the group are all requested before any of
 //     them is consumed (U x (256 B + 512 B) in flight per warp instead of one row);
 //   * runs (duplicates) are handled by carrying the accumulator across entries - run boundaries are a ballot mask, so every branch
-//     is warp-uniform. Accumulation order and fma contraction are those of the generic walk: results are bit-identical.
+//     is warp-uniform. The gradient accumulation order is that of the generic walk, so SGD results are bit-identical to it. Row-wise
+//     Adagrad's square sum of a row is not: the compiler may contract x*x + y*y + ... into a different fma chain here than in
+//     apply_row, so at D <= 128 the row state and the update can differ from the generic walk by rounding (a few ulp).
 // Runs that continue into a neighbouring chunk leave partial rows exactly like the generic walk (span kernels combine them).
 // Chunks it handled are marked in chunk_done; the generic kernel returns immediately for those.
 // Entries in flight per warp vs CTAs per SM (register budget: U x MAXV x 2 float4): D <= 128 (MAXV == 1) walks 2 entries at a time at
@@ -475,7 +477,8 @@ __global__ void __launch_bounds__(256, MAXV == 1 ? 4 : 3) tbe_bwd_walk_kernel(co
     }
     // Group of U DISTINCT rows that all live inside the chunk (the common case for large tables): the U updates are independent, so
     // their square-sum reductions, square roots and divisions are interleaved instead of running as U dependent chains back to back
-    // (with one warp per scheduler-slot nothing else hides that latency). Same arithmetic, same order per row as the sequential path below: bit-identical results.
+    // (with one warp per scheduler-slot nothing else hides that latency). Same operations in the same order per row as the sequential
+    // path below (the square sums may still be contracted differently, see above).
     if constexpr (U > 1) {
       constexpr unsigned kAll = (1u << U) - 1u;
       const bool distinct = j + U <= cnt_v && ((ends >> j) & kAll) == kAll && (j == 0 || ((ends >> (j - 1)) & 1u)) &&
@@ -756,12 +759,16 @@ __global__ void __launch_bounds__(256) tbe_bwd_span_kernel(const TbeBwdParams p)
   apply_row<W, MAXV>(p, (int64_t) rk, f, acc, lane);
 }
 
-// kLongWarps warps per long span: at 8 GPUs the global batch makes the hot rows of the tiny tables 8x longer (a 3-row table: 87 k entries
-// per row = 2730 partial rows), and this kernel runs at the very end of the step.
-constexpr int kLongWarps = 32;
+// long_warps<MAXV>() warps per long span: at 8 GPUs the global batch makes the hot rows of the tiny tables 8x longer (a 3-row table: 87 k
+// entries per row = 2730 partial rows), and this kernel runs at the very end of the step. Each warp leaves one row of max_dim floats in
+// shared memory: 32 warps fit the opt-in limit (227 KiB on H100) up to D = 1816 only, so rows wider than 512 take 16 warps (128 KiB at
+// D = 2048).
+template <int MAXV>
+__host__ __device__ constexpr int long_warps() { return MAXV <= 4 ? 32 : 16; }
 
 template <typename W, int MAXV>
-__global__ void __launch_bounds__(kLongWarps * 32) tbe_bwd_span_long_kernel(const TbeBwdParams p) {
+__global__ void __launch_bounds__(long_warps<MAXV>() * 32) tbe_bwd_span_long_kernel(const TbeBwdParams p) {
+  constexpr int kLongWarps = long_warps<MAXV>();
   extern __shared__ float smem[];  // [kLongWarps][max_dim]
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int n_long = *p.long_count;
@@ -875,6 +882,16 @@ static int run_bwd(TbeBwdParams& p, char* ws, cudaStream_t stream) {
     g_trb_launches += 4;  // radix sort passes (library kernels, counted approximately)
   }
   if (p.phase == 1) return 0;
+  // The long-span kernel's shared memory is checked before the first kernel that updates rows: a shape it cannot run fails with
+  // every row unchanged.
+  const size_t smem = (size_t) long_warps<MAXV>() * p.max_dim * sizeof(float);
+  if (smem > 48 * 1024) {
+    int dev = 0, optin = 0;
+    TRB_CUDA(cudaGetDevice(&dev));
+    TRB_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+    if (smem > (size_t) optin) return -2;
+    TRB_CUDA(cudaFuncSetAttribute(tbe_bwd_span_long_kernel<W, MAXV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem));
+  }
   const int64_t chunks = (p.n + 31) / 32;
   const int64_t blocks = (chunks + 7) / 8;
   // pass 1: SGD / row-wise Adagrad without weight decay or stochastic rounding walk their chunks several entries at a time
@@ -892,10 +909,7 @@ static int run_bwd(TbeBwdParams& p, char* ws, cudaStream_t stream) {
   // pass 3: combine runs that span chunks (warp per flagged chunk), then the few long spans with whole blocks
   tbe_bwd_span_kernel<W, MAXV><<<(unsigned) blocks, threads, 0, stream>>>(p);
   TRB_CHECK_LAUNCH();
-  const size_t smem = (size_t) kLongWarps * p.max_dim * sizeof(float);
-  if (smem > 48 * 1024)
-    TRB_CUDA(cudaFuncSetAttribute(tbe_bwd_span_long_kernel<W, MAXV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem));
-  tbe_bwd_span_long_kernel<W, MAXV><<<trb_num_sms(), kLongWarps * 32, smem, stream>>>(p);
+  tbe_bwd_span_long_kernel<W, MAXV><<<trb_num_sms(), long_warps<MAXV>() * 32, smem, stream>>>(p);
   TRB_CHECK_LAUNCH();
   return 0;
 }
@@ -972,6 +986,7 @@ TRB_API int trb_tbe_bwd_fused(void* weights, int w_dtype, float* state1, float* 
   TRB_BWD_CASE(TRB_BF16, __nv_bfloat16, TRB_F32, float);
   TRB_BWD_CASE(TRB_BF16, __nv_bfloat16, TRB_BF16, __nv_bfloat16);
   TRB_BWD_CASE(TRB_F16, __half, TRB_F32, float);
+  TRB_BWD_CASE(TRB_F16, __half, TRB_BF16, __nv_bfloat16);
 #undef TRB_BWD_CASE
   return -3;
 }

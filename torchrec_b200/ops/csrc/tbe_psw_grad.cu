@@ -99,6 +99,7 @@ TRB_API int trb_tbe_psw_grad(const void* weights, int w_dtype, const int64_t* fe
   PSW_CASE(TRB_BF16, __nv_bfloat16, TRB_F32, float)
   PSW_CASE(TRB_F16, __half, TRB_F16, __half)
   PSW_CASE(TRB_F16, __half, TRB_F32, float)
+  PSW_CASE(TRB_F16, __half, TRB_BF16, __nv_bfloat16)
 #undef PSW_CASE
   return -3;
 }

@@ -89,19 +89,37 @@ def bench_colsum():
     print(f"| total (the 7 bias gradients of one DLRM step) | {tot:.1f} | |")
 
 
+INTERACTION_SHAPES = [(16, 26), (32, 26), (32, 40), (48, 26), (64, 8), (64, 26), (64, 40), (96, 26), (128, 15), (128, 26), (128, 31),
+                      (128, 63), (128, 100), (192, 26), (256, 26), (256, 127)]
+
+
 def bench_interaction():
-    print("| interaction | us | GB moved | GB/s |\n|---|---|---|---|")
-    B, F, D = 32768, 26, 128
-    dense = torch.randn(B, D, device=dev).bfloat16().requires_grad_()
-    sparse = torch.randn(B, F, D, device=dev).bfloat16().requires_grad_()
-    out = I.DotInteractionFn.apply(dense, sparse)
-    g = torch.randn_like(out)
-    us = timeit(lambda: I.DotInteractionFn.apply(dense, sparse))
-    gb = (B * (F + 1) * D * 2 + out.numel() * 2) / 1e9
-    print(f"| fwd B={B} F={F} | {us:.1f} | {gb:.3f} | {gb / us * 1e6:.0f} |")
-    us = timeit(lambda: torch.autograd.grad(out, (dense, sparse), g, retain_graph=True))
-    gb = (2 * B * (F + 1) * D * 2 + out.numel() * 2) / 1e9
-    print(f"| bwd B={B} F={F} | {us:.1f} | {gb:.3f} | {gb / us * 1e6:.0f} |")
+    """Kernel vs the eager PyTorch formulation (ops/dense.py) at B = 32768, bf16. Bytes moved are the least the op must move:
+    fwd reads X [B, F+1, D] and writes the padded output; bwd reads X and the output gradient and writes dX."""
+    from torchrec_b200.ops import dense as DN
+
+    print(f"GPU: {torch.cuda.get_device_name(dev)}")
+    print("| interaction (D, F) | pass | kernel us | eager us | GB moved | kernel GB/s | eager GB/s | eager / kernel |\n|---|---|---|---|---|---|---|---|")
+    B = 32768
+    for D, F in INTERACTION_SHAPES:
+        dense = torch.randn(B, D, device=dev).bfloat16().requires_grad_()
+        sparse = torch.randn(B, F, D, device=dev).bfloat16().requires_grad_()
+        assert I.supported(dense, sparse), (D, F)
+        out = I.DotInteractionFn.apply(dense, sparse)
+        g = torch.randn_like(out)
+        DN.set_dense_backend("torch")
+        out_e = DN.dot_interaction(dense, sparse)
+        g_e = g[:, : out_e.shape[1]].contiguous()
+        x_bytes = B * (F + 1) * D * 2
+        for name, gb, fk, fe in (
+            ("fwd", (x_bytes + out.numel() * 2) / 1e9, lambda: I.DotInteractionFn.apply(dense, sparse), lambda: DN.dot_interaction(dense, sparse)),
+            ("bwd", (2 * x_bytes + out.numel() * 2) / 1e9, lambda: torch.autograd.grad(out, (dense, sparse), g, retain_graph=True),
+             lambda: torch.autograd.grad(out_e, (dense, sparse), g_e, retain_graph=True)),
+        ):
+            uk, ue = timeit(fk), timeit(fe)
+            print(f"| {D}, {F} | {name} | {uk:.1f} | {ue:.1f} | {gb:.3f} | {gb / uk * 1e6:.0f} | {gb / ue * 1e6:.0f} | {ue / uk:.2f} |")
+        del dense, sparse, out, g, out_e, g_e
+        torch.cuda.empty_cache()
 
 
 def bench_tbe(rows_per_table=40_000_000, n_tables=8):

@@ -13,9 +13,13 @@ def _ceil8(x: int) -> int:
 
 
 def supported(dense: torch.Tensor, sparse: torch.Tensor) -> bool:
-    return (dense.is_cuda and dense.dim() == 2 and sparse.dim() == 3 and dense.shape[1] == 128 and sparse.shape[2] == 128
-            and 1 <= sparse.shape[1] <= 31 and sparse.dtype in (torch.float32, torch.bfloat16) and sparse.stride(2) == 1
-            and sparse.stride(1) == 128 and sparse.stride(0) % 8 == 0)
+    """Shapes the kernels cover: D % 16 == 0 with 16 <= D <= 256 and 1 <= F <= 127 (one 128-row MMA tile per sample at most)."""
+    if not (dense.is_cuda and dense.dim() == 2 and sparse.dim() == 3):
+        return False
+    D = dense.shape[1]
+    return (sparse.shape[2] == D and D % 16 == 0 and 16 <= D <= 256 and 1 <= sparse.shape[1] <= 127
+            and sparse.dtype in (torch.float32, torch.bfloat16) and sparse.stride(2) == 1 and sparse.stride(1) == D
+            and sparse.stride(0) % 8 == 0)
 
 
 class DotInteractionFn(torch.autograd.Function):

@@ -269,3 +269,4 @@ def assign_weights_to_tbe(model: torch.nn.Module, table_to_weight: Dict[str, tor
             src = table_to_weight[name]
             assert tuple(src.shape) == tuple(w.shape), f"{name}: got {tuple(src.shape)}, table is {tuple(w.shape)}"
             w.copy_(src.to(w.device))
+        tbe.invalidate_cache()  # host-resident tables behind an HBM row cache: the cached copies are stale now

@@ -8,10 +8,38 @@
 //   FMT_FP8_BLOCK                  : e4m3 values + one fp16 scale per 32-element block ([D bytes][D/32 x fp16])
 // One warp per bag; lane l dequantises elements 4l..4l+3 (+128k), accumulates in fp32, writes fp32/bf16/fp16.
 // Parity: IntNBitTableBatchedEmbeddingBagsCodegen forward (reference quant_embedding_kernel.py:247-711).
+//
+// Placed launches (template PLACED = true, entry point trb_qtbe_fwd_placed): every feature has an absolute row base, so one launch mixes
+// tables in HBM with tables in pinned host memory (UVA: the kernel dereferences the host pointer, zero-copy over the host link). A host
+// table may sit behind an HBM row cache: the row address is `slot >= 0 ? cache + slot * rb : host + id * rb`. A miss is served from host
+// memory in the same kernel and claims the row for admission (slot map ABSENT -> PENDING, one claimant per row, appended to a bounded
+// miss list); trb_qcache_admit then copies the claimed rows into slots picked by CLOCK. Serving tables are read-only, so an eviction
+// never writes back, and what the cache holds never changes a result. The all-HBM launch (trb_qtbe_fwd_ex) runs the PLACED = false
+// instances, which compile to exactly the kernels without placement.
 #include "common.cuh"
 #include <cuda_fp8.h>
+#include <cstring>
+#include <type_traits>
 
 enum QFmt : int { FMT_FP32 = 0, FMT_FP16 = 1, FMT_BF16 = 2, FMT_INT8 = 3, FMT_INT4 = 4, FMT_INT2 = 5, FMT_FP8_BLOCK = 6 };
+
+constexpr int32_t QC_ABSENT = -1;   // slot map: row not cached
+constexpr int32_t QC_PENDING = -2;  // slot map: row claimed for admission by a lookup of this call
+
+// One cached table (an array of these lives in device memory; ops/quant_tbe.py packs it as int64 words, field order matters).
+struct QCacheTab {
+  int32_t* slot_of_row;        // [rows] cache slot of a row, QC_ABSENT or QC_PENDING
+  int64_t* row_of_slot;        // [slots] row held by a slot, -1 when empty
+  uint8_t* ref;                // [slots] CLOCK reference bits (set by hits and by admission)
+  uint8_t* cache;              // [slots, rb] cached rows (HBM)
+  const uint8_t* host;         // [rows, rb] the table (pinned host memory)
+  int64_t* miss;               // [cap] rows claimed by the lookups of one call
+  int64_t* victim;             // [cap] slot picked for miss[i]
+  int32_t* ctr;                // [2] claims of the current call (may exceed cap), admissions of the last admission call
+  int64_t* hand;               // [1] CLOCK hand
+  unsigned long long* stats;   // [4] lookups, hits, admissions, evictions
+  int64_t slots, cap, rb;
+};
 
 struct QTbeParams {
   const uint8_t* weights;
@@ -27,6 +55,79 @@ struct QTbeParams {
   void* out;
   int64_t out_stride;
   int32_t B, F, idx64, off64, mean, pooled;
+};
+
+// Parameters of a placed launch (weights / feat_woff unused there). A separate type, so the parameter block of the all-HBM kernels stays
+// as it was: growing it changed their register allocation and spills.
+struct QTbePlaced : QTbeParams {
+  const int64_t* feat_base;   // address of row 0 of the feature's table (HBM or pinned host)
+  const int32_t* feat_ctab;    // cached table of the feature, -1 when its rows are not cached
+  const QCacheTab* ctabs;
+  const int32_t* no_slot;      // one QC_ABSENT word: the slot-map load of an uncached feature
+};
+
+template <bool PLACED> using QP = std::conditional_t<PLACED, QTbePlaced, QTbeParams>;
+
+// Where a placed bag reads its rows from.
+struct QPlace {
+  const uint8_t* base;
+  const uint8_t* cache;
+  const int32_t* smap;
+  int ct;
+};
+
+__device__ __forceinline__ QPlace qplace(const QTbePlaced& p, int f) {
+  QPlace q;
+  q.base = reinterpret_cast<const uint8_t*>(p.feat_base[f]);
+  q.ct = p.feat_ctab[f];
+  if (q.ct >= 0) {
+    q.cache = p.ctabs[q.ct].cache;
+    q.smap = p.ctabs[q.ct].slot_of_row;
+  } else {
+    q.cache = q.base;
+    q.smap = p.no_slot;
+  }
+  return q;
+}
+
+// Row `idx` (already clamped into the table) of a placed bag. The slot is an unconditional load (an uncached feature reads the constant
+// QC_ABSENT word) and the select is on the address, never on loaded row data.
+__device__ __forceinline__ const uint8_t* qrow(const QPlace& q, int64_t idx, int64_t rb, int32_t& slot) {
+  slot = q.smap[q.ct >= 0 ? idx : 0];
+  return slot >= 0 ? q.cache + (int64_t) slot * rb : q.base + idx * rb;
+}
+
+// Cache bookkeeping of one valid lookup of a cached table: a hit sets the slot's reference bit; a miss on an absent row claims it and
+// appends it to the miss list (a claim that does not fit returns the row to ABSENT, so a later call can admit it).
+__device__ __forceinline__ void qcache_note(const QCacheTab& t, int64_t idx, int32_t slot) {
+  if (slot >= 0) {
+    if (!t.ref[slot]) t.ref[slot] = 1;
+  } else if (slot == QC_ABSENT && atomicCAS(t.slot_of_row + idx, QC_ABSENT, QC_PENDING) == QC_ABSENT) {
+    const int32_t pos = atomicAdd(t.ctr, 1);
+    if (pos < t.cap) t.miss[pos] = idx;
+    else atomicExch(t.slot_of_row + idx, QC_ABSENT);
+  }
+}
+
+// Per-thread lookup / hit counts of the cached table being served, flushed when the table changes and when the thread ends.
+struct QCount {
+  int ct = -1;
+  unsigned long long lookups = 0, hits = 0;
+  __device__ __forceinline__ void flush(const QCacheTab* tabs) {
+    if (ct >= 0 && lookups) {
+      atomicAdd(tabs[ct].stats, lookups);
+      if (hits) atomicAdd(tabs[ct].stats + 1, hits);
+    }
+    lookups = hits = 0;
+  }
+  __device__ __forceinline__ void add(const QCacheTab* tabs, int c, int32_t slot) {
+    if (c != ct) {
+      flush(tabs);
+      ct = c;
+    }
+    ++lookups;
+    hits += slot >= 0;
+  }
 };
 
 __device__ __forceinline__ float4 dequant4(const uint8_t* row, int fmt, int D, int e) {
@@ -64,8 +165,8 @@ __device__ __forceinline__ float4 dequant4(const uint8_t* row, int fmt, int D, i
   return make_float4(0.f, 0.f, 0.f, 0.f);
 }
 
-template <typename O, int MAXV>
-__global__ void __launch_bounds__(256) qtbe_fwd_kernel(const QTbeParams p) {
+template <typename O, int MAXV, bool PLACED>
+__global__ void __launch_bounds__(256) qtbe_fwd_kernel(const QP<PLACED> p) {
   const int lane = threadIdx.x & 31;
   const int64_t bag = ((int64_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int64_t n_bags = (int64_t) p.F * p.B;
@@ -77,7 +178,11 @@ __global__ void __launch_bounds__(256) qtbe_fwd_kernel(const QTbeParams p) {
   const int fmt = p.feat_fmt[f];
   const int64_t rows = p.feat_rows[f];
   const int64_t rb = p.feat_row_bytes[f];
-  const uint8_t* wbase = p.weights + p.feat_woff[f];
+  const uint8_t* wbase;
+  QPlace pl;
+  QCount cnt;
+  if constexpr (PLACED) pl = qplace(p, f);
+  else wbase = p.weights + p.feat_woff[f];
   const int64_t start = trb_ld_idx(p.offsets, bag, p.off64);
   const int64_t end = trb_ld_idx(p.offsets, bag + 1, p.off64);
   float4 acc[MAXV];
@@ -87,15 +192,32 @@ __global__ void __launch_bounds__(256) qtbe_fwd_kernel(const QTbeParams p) {
     const int n = (int) min((int64_t) 32, end - l0);
     int64_t my_idx = 0;
     float my_w = 0.f;
+    const uint8_t* my_row = nullptr;
     if (lane < n) {
       my_idx = trb_ld_idx(p.indices, l0 + lane, p.idx64);
       my_w = p.psw ? p.psw[l0 + lane] : 1.f;
-      if (my_idx < 0 || my_idx >= rows) { my_idx = 0; my_w = 0.f; }
+      const bool ok = my_idx >= 0 && my_idx < rows;
+      if (!ok) { my_idx = 0; my_w = 0.f; }
+      if constexpr (PLACED) {  // every lane resolves the row of its own id; the bag loop below shuffles the address
+        int32_t slot;
+        my_row = qrow(pl, my_idx, rb, slot);
+        if (ok && pl.ct >= 0) {
+          qcache_note(p.ctabs[pl.ct], my_idx, slot);
+          cnt.add(p.ctabs, pl.ct, slot);
+        }
+      }
     }
     for (int j = 0; j < n; ++j) {
-      const int64_t idx = __shfl_sync(0xffffffffu, my_idx, j);
-      const float w = __shfl_sync(0xffffffffu, my_w, j);
-      const uint8_t* row = wbase + idx * rb;
+      const uint8_t* row;
+      float w;
+      if constexpr (PLACED) {
+        row = reinterpret_cast<const uint8_t*>(__shfl_sync(0xffffffffu, reinterpret_cast<unsigned long long>(my_row), j));
+        w = __shfl_sync(0xffffffffu, my_w, j);
+      } else {
+        const int64_t idx = __shfl_sync(0xffffffffu, my_idx, j);
+        w = __shfl_sync(0xffffffffu, my_w, j);
+        row = wbase + idx * rb;
+      }
 #pragma unroll
       for (int k = 0; k < MAXV; ++k) {
         const int vi = lane + k * 32;
@@ -114,6 +236,7 @@ __global__ void __launch_bounds__(256) qtbe_fwd_kernel(const QTbeParams p) {
     const int vi = lane + k * 32;
     if (vi < nvec) Vec4<O>::st(dst + vi * 4, acc[k]);
   }
+  if constexpr (PLACED) cnt.flush(p.ctabs);
 }
 
 // ---- vector fast path (every table of the launch in ONE of INT8 / FP8 block-scaled / FP16 / BF16 / INT4) -----------------------------
@@ -184,8 +307,8 @@ __device__ __forceinline__ void store_vec(O* dst, const float (&a)[N]) {
   for (int k = 0; k < N / 4; ++k) Vec4<O>::st(dst + 4 * k, make_float4(a[4 * k], a[4 * k + 1], a[4 * k + 2], a[4 * k + 3]));
 }
 
-template <typename O, int FMT, int MAXV, int U>
-__global__ void __launch_bounds__(256, 3) qtbe_fwd_vec_kernel(const QTbeParams p) {
+template <typename O, int FMT, int MAXV, int U, bool PLACED>
+__global__ void __launch_bounds__(256, 3) qtbe_fwd_vec_kernel(const QP<PLACED> p) {
   constexpr int LPR = 8;
   constexpr int EPV = QVec<FMT>::EPV;
   const int lig = threadIdx.x & (LPR - 1);
@@ -195,6 +318,7 @@ __global__ void __launch_bounds__(256, 3) qtbe_fwd_vec_kernel(const QTbeParams p
   if (bag0 >= n_bags) return;
   int64_t st[U], en[U];
   const uint8_t* wb[U];
+  QPlace pl[U];
   int64_t rb[U], rows[U];
   int D[U], col[U], b_of[U];
 #pragma unroll
@@ -206,7 +330,12 @@ __global__ void __launch_bounds__(256, 3) qtbe_fwd_vec_kernel(const QTbeParams p
     col[u] = p.feat_col[f];
     rows[u] = p.feat_rows[f];
     rb[u] = p.feat_row_bytes[f];
-    wb[u] = p.weights + p.feat_woff[f];
+    if constexpr (PLACED) {
+      pl[u] = qplace(p, f);
+      wb[u] = pl[u].base;
+    } else {
+      wb[u] = p.weights + p.feat_woff[f];
+    }
     st[u] = trb_ld_idx(p.offsets, bag, p.off64);
     en[u] = bag0 + u < n_bags ? trb_ld_idx(p.offsets, bag + 1, p.off64) : st[u];
   }
@@ -215,15 +344,23 @@ __global__ void __launch_bounds__(256, 3) qtbe_fwd_vec_kernel(const QTbeParams p
   uint32_t sw[U][MAXV];
   float w0[U];
   const uint8_t* row0[U];
+  int64_t idx0[U];   // placed: the valid first id of the bag (-1: none) and its slot, noted after every load is issued
+  int32_t slot0[U];
 #pragma unroll
   for (int u = 0; u < U; ++u) {
     w0[u] = 0.f;
     row0[u] = wb[u];
+    if constexpr (PLACED) idx0[u] = -1;
     if (en[u] > st[u]) {
       const int64_t idx = trb_ld_idx(p.indices, st[u], p.idx64);
       if (idx >= 0 && idx < rows[u]) {
         w0[u] = p.psw ? p.psw[st[u]] : 1.f;
-        row0[u] = wb[u] + idx * rb[u];
+        if constexpr (PLACED) {
+          row0[u] = qrow(pl[u], idx, rb[u], slot0[u]);
+          idx0[u] = idx;
+        } else {
+          row0[u] = wb[u] + idx * rb[u];
+        }
       }
     }
 #pragma unroll
@@ -234,6 +371,18 @@ __global__ void __launch_bounds__(256, 3) qtbe_fwd_vec_kernel(const QTbeParams p
       const int vc = vi * EPV < D[u] ? vi : 0;
       q[u][k] = *reinterpret_cast<const uint4*>(row0[u] + vc * 16);
       sw[u][k] = load_scale_vec<FMT>(row0[u], D[u], vc * EPV);
+    }
+  }
+  QCount cnt;
+  if constexpr (PLACED) {
+    if (lig == 0) {  // one lane of the 8 owning a bag keeps its books
+#pragma unroll
+      for (int u = 0; u < U; ++u) {
+        if (idx0[u] >= 0 && pl[u].ct >= 0) {
+          qcache_note(p.ctabs[pl[u].ct], idx0[u], slot0[u]);
+          cnt.add(p.ctabs, pl[u].ct, slot0[u]);
+        }
+      }
     }
   }
 #pragma unroll
@@ -258,7 +407,17 @@ __global__ void __launch_bounds__(256, 3) qtbe_fwd_vec_kernel(const QTbeParams p
       const int64_t idx = trb_ld_idx(p.indices, j, p.idx64);
       if (idx < 0 || idx >= rows[u]) continue;
       const float w = p.psw ? p.psw[j] : 1.f;
-      const uint8_t* row = wb[u] + idx * rb[u];
+      const uint8_t* row;
+      if constexpr (PLACED) {
+        int32_t slot;
+        row = qrow(pl[u], idx, rb[u], slot);
+        if (lig == 0 && pl[u].ct >= 0) {
+          qcache_note(p.ctabs[pl[u].ct], idx, slot);
+          cnt.add(p.ctabs, pl[u].ct, slot);
+        }
+      } else {
+        row = wb[u] + idx * rb[u];
+      }
 #pragma unroll
       for (int k = 0; k < MAXV; ++k) {
         const int vi = lig + k * LPR;
@@ -286,10 +445,11 @@ __global__ void __launch_bounds__(256, 3) qtbe_fwd_vec_kernel(const QTbeParams p
       }
     }
   }
+  if constexpr (PLACED) cnt.flush(p.ctabs);
 }
 
-template <typename O, int FMT>
-static int launch_q_vec(const QTbeParams& p, int max_dim, cudaStream_t stream) {
+template <typename O, int FMT, bool PLACED>
+static int launch_q_vec(const QP<PLACED>& p, int max_dim, cudaStream_t stream) {
   const int64_t n_bags = (int64_t) p.F * p.B;
   if (n_bags == 0) return 0;
   const int threads = 256;
@@ -298,7 +458,7 @@ static int launch_q_vec(const QTbeParams& p, int max_dim, cudaStream_t stream) {
   {                                                                                                           \
     const int64_t groups = (n_bags + U - 1) / U;                                                              \
     const unsigned blocks = (unsigned) ((groups * 8 + threads - 1) / threads);                                \
-    qtbe_fwd_vec_kernel<O, FMT, MAXV, U><<<blocks, threads, 0, stream>>>(p);                                  \
+    qtbe_fwd_vec_kernel<O, FMT, MAXV, U, PLACED><<<blocks, threads, 0, stream>>>(p);                          \
   }
   if (vecs <= 8) TRB_QVEC(1, 4)
   else if (vecs <= 16) TRB_QVEC(2, 2)
@@ -310,8 +470,8 @@ static int launch_q_vec(const QTbeParams& p, int max_dim, cudaStream_t stream) {
 }
 
 // sequence (unpooled): one warp per id position
-template <typename O>
-__global__ void __launch_bounds__(256) qtbe_seq_kernel(const QTbeParams p, int64_t total) {
+template <typename O, bool PLACED>
+__global__ void __launch_bounds__(256) qtbe_seq_kernel(const QP<PLACED> p, int64_t total) {
   const int lane = threadIdx.x & 31;
   const int64_t i = ((int64_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   if (i >= total) return;
@@ -325,7 +485,20 @@ __global__ void __launch_bounds__(256) qtbe_seq_kernel(const QTbeParams p, int64
   const int nvec = D >> 2;
   int64_t idx = trb_ld_idx(p.indices, i, p.idx64);
   const bool ok = idx >= 0 && idx < p.feat_rows[f];
-  const uint8_t* row = p.weights + p.feat_woff[f] + (ok ? idx : 0) * (int64_t) p.feat_row_bytes[f];
+  const uint8_t* row;
+  if constexpr (PLACED) {
+    const QPlace pl = qplace(p, f);
+    int32_t slot;
+    row = qrow(pl, ok ? idx : 0, p.feat_row_bytes[f], slot);
+    if (lane == 0 && ok && pl.ct >= 0) {
+      qcache_note(p.ctabs[pl.ct], idx, slot);
+      QCount cnt;
+      cnt.add(p.ctabs, pl.ct, slot);
+      cnt.flush(p.ctabs);
+    }
+  } else {
+    row = p.weights + p.feat_woff[f] + (ok ? idx : 0) * (int64_t) p.feat_row_bytes[f];
+  }
   O* dst = reinterpret_cast<O*>(p.out) + i * p.out_stride;
   for (int vi = lane; vi < nvec; vi += 32) {
     float4 v = ok ? dequant4(row, p.feat_fmt[f], D, vi * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
@@ -333,19 +506,19 @@ __global__ void __launch_bounds__(256) qtbe_seq_kernel(const QTbeParams p, int64
   }
 }
 
-template <typename O>
-static int launch_q(const QTbeParams& p, int max_dim, int64_t total, int uniform_fmt, cudaStream_t stream) {
+template <typename O, bool PLACED>
+static int launch_q(const QP<PLACED>& p, int max_dim, int64_t total, int uniform_fmt, cudaStream_t stream) {
   const int threads = 256;
   if (p.pooled && uniform_fmt >= 0) {  // (the caller guarantees rows made of whole 16-byte vectors: quant_tbe.py _uniform_fmt)
-    if (uniform_fmt == FMT_FP8_BLOCK && max_dim <= 512) return launch_q_vec<O, FMT_FP8_BLOCK>(p, max_dim, stream);
-    if (uniform_fmt == FMT_INT8 && max_dim <= 512) return launch_q_vec<O, FMT_INT8>(p, max_dim, stream);
-    if (uniform_fmt == FMT_FP16 && max_dim <= 256) return launch_q_vec<O, FMT_FP16>(p, max_dim, stream);
-    if (uniform_fmt == FMT_BF16 && max_dim <= 256) return launch_q_vec<O, FMT_BF16>(p, max_dim, stream);
-    if (uniform_fmt == FMT_INT4 && max_dim <= 1024) return launch_q_vec<O, FMT_INT4>(p, max_dim, stream);
+    if (uniform_fmt == FMT_FP8_BLOCK && max_dim <= 512) return launch_q_vec<O, FMT_FP8_BLOCK, PLACED>(p, max_dim, stream);
+    if (uniform_fmt == FMT_INT8 && max_dim <= 512) return launch_q_vec<O, FMT_INT8, PLACED>(p, max_dim, stream);
+    if (uniform_fmt == FMT_FP16 && max_dim <= 256) return launch_q_vec<O, FMT_FP16, PLACED>(p, max_dim, stream);
+    if (uniform_fmt == FMT_BF16 && max_dim <= 256) return launch_q_vec<O, FMT_BF16, PLACED>(p, max_dim, stream);
+    if (uniform_fmt == FMT_INT4 && max_dim <= 1024) return launch_q_vec<O, FMT_INT4, PLACED>(p, max_dim, stream);
   }
   if (!p.pooled) {
     if (total == 0) return 0;
-    qtbe_seq_kernel<O><<<(unsigned) ((total * 32 + threads - 1) / threads), threads, 0, stream>>>(p, total);
+    qtbe_seq_kernel<O, PLACED><<<(unsigned) ((total * 32 + threads - 1) / threads), threads, 0, stream>>>(p, total);
     TRB_CHECK_LAUNCH();
     return 0;
   }
@@ -353,12 +526,22 @@ static int launch_q(const QTbeParams& p, int max_dim, int64_t total, int uniform
   if (n_bags == 0) return 0;
   const unsigned blocks = (unsigned) ((n_bags * 32 + threads - 1) / threads);
   const int nvec = max_dim / 4;
-  if (nvec <= 32) qtbe_fwd_kernel<O, 1><<<blocks, threads, 0, stream>>>(p);
-  else if (nvec <= 128) qtbe_fwd_kernel<O, 4><<<blocks, threads, 0, stream>>>(p);
-  else if (nvec <= 512) qtbe_fwd_kernel<O, 16><<<blocks, threads, 0, stream>>>(p);
+  if (nvec <= 32) qtbe_fwd_kernel<O, 1, PLACED><<<blocks, threads, 0, stream>>>(p);
+  else if (nvec <= 128) qtbe_fwd_kernel<O, 4, PLACED><<<blocks, threads, 0, stream>>>(p);
+  else if (nvec <= 512) qtbe_fwd_kernel<O, 16, PLACED><<<blocks, threads, 0, stream>>>(p);
   else return -2;
   TRB_CHECK_LAUNCH();
   return 0;
+}
+
+template <bool PLACED>
+static int launch_q_out(const QP<PLACED>& p, int out_dtype, int max_dim, int64_t total, int uniform_fmt, cudaStream_t stream) {
+  switch (out_dtype) {
+    case TRB_F32: return launch_q<float, PLACED>(p, max_dim, total, uniform_fmt, stream);
+    case TRB_F16: return launch_q<__half, PLACED>(p, max_dim, total, uniform_fmt, stream);
+    case TRB_BF16: return launch_q<__nv_bfloat16, PLACED>(p, max_dim, total, uniform_fmt, stream);
+  }
+  return -3;
 }
 
 TRB_API int trb_qtbe_fwd_ex(const void* weights, const int64_t* feat_woff, const int64_t* feat_rows, const int32_t* feat_dim, const int32_t* feat_col,
@@ -379,15 +562,140 @@ TRB_API int trb_qtbe_fwd_ex(const void* weights, const int64_t* feat_woff, const
                             const int32_t* feat_fmt, const int32_t* feat_row_bytes, const void* indices, int idx64, const void* offsets, int off64,
                             const float* psw, void* out, int out_dtype, int64_t out_stride, int B, int F, int max_dim, int mean, int pooled,
                             int64_t total, int uniform_fmt, cudaStream_t stream) {
-  QTbeParams p;
+  QTbeParams p{};
   p.weights = reinterpret_cast<const uint8_t*>(weights);
   p.feat_woff = feat_woff; p.feat_rows = feat_rows; p.feat_dim = feat_dim; p.feat_col = feat_col; p.feat_fmt = feat_fmt;
   p.feat_row_bytes = feat_row_bytes; p.indices = indices; p.offsets = offsets; p.psw = psw; p.out = out; p.out_stride = out_stride;
   p.B = B; p.F = F; p.idx64 = idx64; p.off64 = off64; p.mean = mean; p.pooled = pooled;
-  switch (out_dtype) {
-    case TRB_F32: return launch_q<float>(p, max_dim, total, uniform_fmt, stream);
-    case TRB_F16: return launch_q<__half>(p, max_dim, total, uniform_fmt, stream);
-    case TRB_BF16: return launch_q<__nv_bfloat16>(p, max_dim, total, uniform_fmt, stream);
+  return launch_q_out<false>(p, out_dtype, max_dim, total, uniform_fmt, stream);
+}
+
+// The same lookup over placed tables: `feat_base` = absolute address of row 0 of each feature's table (HBM or pinned host memory),
+// `feat_ctab` = index into `ctabs` of the feature's HBM row cache or -1, `no_slot` = one device word holding QC_ABSENT (-1).
+TRB_API int trb_qtbe_fwd_placed(const int64_t* feat_base, const int32_t* feat_ctab, const void* ctabs, const int32_t* no_slot, const int64_t* feat_rows,
+                                const int32_t* feat_dim, const int32_t* feat_col, const int32_t* feat_fmt, const int32_t* feat_row_bytes, const void* indices,
+                                int idx64, const void* offsets, int off64, const float* psw, void* out, int out_dtype, int64_t out_stride, int B, int F,
+                                int max_dim, int mean, int pooled, int64_t total, int uniform_fmt, cudaStream_t stream) {
+  QTbePlaced p{};
+  p.feat_base = feat_base; p.feat_ctab = feat_ctab; p.ctabs = reinterpret_cast<const QCacheTab*>(ctabs); p.no_slot = no_slot;
+  p.feat_rows = feat_rows; p.feat_dim = feat_dim; p.feat_col = feat_col; p.feat_fmt = feat_fmt;
+  p.feat_row_bytes = feat_row_bytes; p.indices = indices; p.offsets = offsets; p.psw = psw; p.out = out; p.out_stride = out_stride;
+  p.B = B; p.F = F; p.idx64 = idx64; p.off64 = off64; p.mean = mean; p.pooled = pooled;
+  return launch_q_out<true>(p, out_dtype, max_dim, total, uniform_fmt, stream);
+}
+
+// ---- admission: claimed misses -> HBM slots ---------------------------------------------------------------------------------------------
+// One block per cached table picks the victims with CLOCK (second chance; one hand per table): the hand sweeps windows of up to 256
+// slots, a slot with a clear reference bit is a victim, a set bit is cleared as the hand passes it. Admitted slots get their bit set, so
+// a second lap clears them instead of taking them again: with at most `slots` admissions per call (cap <= slots) no slot is taken twice.
+__global__ void __launch_bounds__(256) qcache_pick_kernel(const QCacheTab* tabs) {
+  const QCacheTab t = tabs[blockIdx.x];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  __shared__ int s_n, s_wcnt[8], s_stop;
+  __shared__ unsigned long long s_evict;
+  if (tid == 0) {
+    s_n = (int) min((int64_t) *t.ctr, t.cap);
+    s_evict = 0;
   }
-  return -3;
+  __syncthreads();
+  const int n = s_n;
+  const int width = (int) min((int64_t) blockDim.x, t.slots);
+  int64_t hand = *t.hand;
+  int taken = 0;
+  while (taken < n) {
+    const int64_t s = (hand + tid) % t.slots;
+    const bool active = tid < width;
+    const bool cand = active && t.ref[s] == 0;
+    const unsigned bal = __ballot_sync(0xffffffffu, cand);
+    if (lane == 0) s_wcnt[warp] = __popc(bal);
+    if (tid == 0) s_stop = width;
+    __syncthreads();
+    int before = 0, total = 0;
+    for (int w = 0; w < 8; ++w) {
+      before += w < warp ? s_wcnt[w] : 0;
+      total += s_wcnt[w];
+    }
+    const int rank = before + __popc(bal & ((1u << lane) - 1u));
+    const int want = n - taken;
+    if (cand && rank == want - 1) s_stop = tid + 1;  // the hand stops right after the last victim it needs
+    __syncthreads();
+    const int stop = s_stop;
+    if (tid < stop) {
+      if (cand) {
+        t.victim[taken + rank] = s;
+        t.ref[s] = 1;  // taken: a later window of this call (the hand can wrap) sees it as referenced
+      } else if (active) {
+        t.ref[s] = 0;
+      }
+    }
+    taken += min(total, want);
+    hand = (hand + stop) % t.slots;
+    __syncthreads();
+  }
+  // retire the victims' rows, hand the slots to the claimed rows (the copy and the slot-map update follow in qcache_fill_kernel)
+  unsigned long long ev = 0;
+  for (int i = tid; i < n; i += blockDim.x) {
+    const int64_t s = t.victim[i];
+    const int64_t old = t.row_of_slot[s];
+    if (old >= 0) {
+      t.slot_of_row[old] = QC_ABSENT;
+      ++ev;
+    }
+    t.row_of_slot[s] = t.miss[i];
+    t.ref[s] = 1;
+  }
+  if (ev) atomicAdd(&s_evict, ev);
+  __syncthreads();
+  if (tid == 0) {
+    *t.hand = hand;
+    t.ctr[0] = 0;
+    t.ctr[1] = n;
+    t.stats[2] += (unsigned long long) n;
+    t.stats[3] += s_evict;
+  }
+}
+
+// One warp per admitted row: host row -> HBM slot in 16-byte vectors, then the row becomes visible to lookups.
+__global__ void __launch_bounds__(256) qcache_fill_kernel(const QCacheTab* tabs) {
+  const QCacheTab& t = tabs[blockIdx.y];
+  const int lane = threadIdx.x & 31;
+  const int64_t i = (int64_t) blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (i >= t.ctr[1]) return;
+  const int64_t row = t.miss[i], slot = t.victim[i];
+  const uint4* src = reinterpret_cast<const uint4*>(t.host + row * t.rb);
+  uint4* dst = reinterpret_cast<uint4*>(t.cache + slot * t.rb);
+  for (int64_t v = lane; v < t.rb / 16; v += 32) dst[v] = src[v];
+  __syncwarp();
+  if (lane == 0) {
+    __threadfence();
+    t.slot_of_row[row] = (int32_t) slot;
+  }
+}
+
+// `tabs`: device array of `n_tabs` QCacheTab; `max_cap`: the largest miss-list capacity among them (grid of the copy). Everything the
+// admission needs stays on the device, so a lookup followed by its admission can be captured in a CUDA graph.
+TRB_API int trb_qcache_admit(const void* tabs, int n_tabs, int64_t max_cap, cudaStream_t stream) {
+  if (n_tabs <= 0 || max_cap <= 0) return 0;
+  const QCacheTab* t = reinterpret_cast<const QCacheTab*>(tabs);
+  qcache_pick_kernel<<<n_tabs, 256, 0, stream>>>(t);
+  TRB_CHECK_LAUNCH();
+  qcache_fill_kernel<<<dim3((unsigned) ((max_cap + 7) / 8), (unsigned) n_tabs), 256, 0, stream>>>(t);
+  TRB_CHECK_LAUNCH();
+  return 0;
+}
+
+// ---- host tables ------------------------------------------------------------------------------------------------------------------------
+// Pinned, mapped, portable host memory of exactly `bytes` bytes (zeroed): the caching pinned allocator of PyTorch rounds a request up to a
+// power of two, which for a 40 GB table pins 64 GB. With UVA the host pointer is also the device pointer on every device.
+TRB_API int trb_host_alloc(int64_t bytes, void** out) {
+  *out = nullptr;
+  if (bytes <= 0) return 0;
+  TRB_CUDA(cudaHostAlloc(out, (size_t) bytes, cudaHostAllocPortable | cudaHostAllocMapped));
+  std::memset(*out, 0, (size_t) bytes);
+  return 0;
+}
+
+TRB_API int trb_host_free(void* p) {
+  if (p) TRB_CUDA(cudaFreeHost(p));
+  return 0;
 }

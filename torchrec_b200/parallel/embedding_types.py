@@ -52,6 +52,28 @@ def compute_kernel_to_embedding_location(compute_kernel: EmbeddingComputeKernel)
     return "managed_caching"
 
 
+_QUANT_KERNELS = (EmbeddingComputeKernel.QUANT, EmbeddingComputeKernel.QUANT_UVM, EmbeddingComputeKernel.QUANT_UVM_CACHING)
+
+
+def quant_table_placement(compute_kernel: Any, cache_params: Any = None, fused_params: Optional[Dict[str, Any]] = None) -> Tuple[Any, float]:
+    """(``EmbeddingLocation``, cache load factor) of a quantized inference table planned with ``compute_kernel``: ``quant`` -> HBM,
+    ``quant_uvm`` -> pinned host memory, ``quant_uvm_caching`` -> pinned host memory + HBM row cache. The load factor comes from
+    ``cache_params.load_factor``, then ``fused_params["cache_load_factor"]``, then the planner's default (the order of the training
+    lookup engine)."""
+    from ..ops.tbe import EmbeddingLocation
+    from .planner.constants import UVM_CACHING_RATIO
+
+    ck = EmbeddingComputeKernel(compute_kernel) if isinstance(compute_kernel, str) else compute_kernel
+    loc = EmbeddingLocation.DEVICE
+    if ck in _QUANT_KERNELS:
+        loc = {"device": EmbeddingLocation.DEVICE, "managed": EmbeddingLocation.MANAGED,
+               "managed_caching": EmbeddingLocation.MANAGED_CACHING}[compute_kernel_to_embedding_location(ck)]
+    clf = getattr(cache_params, "load_factor", None) if cache_params is not None else None
+    if not clf:
+        clf = (fused_params or {}).get("cache_load_factor")
+    return loc, float(clf) if clf else UVM_CACHING_RATIO
+
+
 class KJTList(Multistreamable):
     """List of KJTs (one per sharding group) that crosses streams together."""
 

@@ -9,7 +9,7 @@ from torch import nn
 
 from ..quant.embedding_modules import EmbeddingCollection as QuantEmbeddingCollection
 from ..sparse.jagged_tensor import JaggedTensor, KeyedJaggedTensor
-from .embedding_types import BaseQuantEmbeddingSharder
+from .embedding_types import BaseQuantEmbeddingSharder, quant_table_placement
 from .engine import shards_of
 from .types import LazyNoWait, NoWait, NullShardedModuleContext, ParameterSharding, ShardedModule, ShardingEnv, ShardingType
 
@@ -45,20 +45,27 @@ class ShardedQuantEmbeddingCollection(ShardedModule[List[KeyedJaggedTensor], Lis
         for (r, cols), units in sorted(groups.items(), key=lambda kv: kv[0]):
             dev = torch.device("cuda", r) if self._device_type == "cuda" else torch.device("cpu")
             shard_keys: List[tuple] = []
-            specs = []
+            specs, locs, clfs = [], [], []
             for f, ti, sh in units:
                 key = (ti, sh.row_off, sh.col_off)
                 if key not in shard_keys:
                     shard_keys.append(key)
                     specs.append((f"{tables[ti].name}_{sh.row_off}_{sh.col_off}", sh.rows, sh.cols, tables[ti].data_type))
+                    ps = params[tables[ti].name]
+                    loc, clf = quant_table_placement(ps.compute_kernel, getattr(ps, "cache_params", None), fused_params)
+                    locs.append(loc)
+                    clfs.append(clf)
             fmap = [shard_keys.index((ti, sh.row_off, sh.col_off)) for _, ti, sh in units]
-            tbe = QuantTableBatchedEmbeddingBags(specs, fmap, pooling_mode=2, output_dtype=self._out_dtype, device=dev)
+            tbe = QuantTableBatchedEmbeddingBags(specs, fmap, pooling_mode=2, output_dtype=self._out_dtype, device=dev, locations=locs,
+                                                 cache_load_factor=clfs)
             for k, (ti, r0, c0) in enumerate(shard_keys):
                 t = tables[ti]
                 src = module.embeddings[t.name].weight
                 rows_k, cols_k = specs[k][1], specs[k][2]
                 if r0 == 0 and c0 == 0 and rows_k == t.num_embeddings and cols_k == t.embedding_dim:
-                    tbe.split_embedding_weights()[k].copy_(src.to(dev))  # whole table: the quantized bytes as they are
+                    dst = tbe.split_embedding_weights()[k]  # whole table: the quantized bytes as they are
+                    dst.copy_(src.to(dst.device))
+                    tbe.invalidate_cache(k)
                 else:  # a rectangle of the table: re-quantized (row scales of column slices differ from the full row's)
                     full = dequantize_rows(src.to("cpu"), t.embedding_dim, t.data_type)
                     tbe.assign_from_float(k, full[r0 : r0 + rows_k, c0 : c0 + cols_k])

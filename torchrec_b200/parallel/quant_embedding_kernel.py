@@ -18,7 +18,7 @@ from ..modules.embedding_configs import DataType, PoolingType, data_type_to_dtyp
 from ..ops.quant_tbe import QuantTableBatchedEmbeddingBags, dequantize_rows, quantize_rows, row_bytes
 from ..sparse.jagged_tensor import KeyedJaggedTensor
 from .embedding_kernel import BaseEmbedding, get_state_dict
-from .embedding_types import GroupedEmbeddingConfig, ShardedEmbeddingTable
+from .embedding_types import GroupedEmbeddingConfig, ShardedEmbeddingTable, quant_table_placement
 
 
 def _copy_config(original: GroupedEmbeddingConfig, data_type: DataType, sparse_type: Any = None, device: Optional[torch.device] = None) -> GroupedEmbeddingConfig:
@@ -80,10 +80,14 @@ class _QuantBase(BaseEmbedding):
         if isinstance(out_dtype, DataType):
             out_dtype = data_type_to_dtype(out_dtype)
         mode = 2 if not self._POOLED else (1 if config.pooling == PoolingType.MEAN else 0)
+        # per table: HBM / pinned host / pinned host + HBM row cache, from the table's compute kernel (quant / quant_uvm / quant_uvm_caching)
+        placement = [quant_table_placement(t.compute_kernel, None, {**(fused_params or {}), **(config.fused_params or {}), **(t.fused_params or {})})
+                     for t in config.embedding_tables]
         self._emb_module = QuantTableBatchedEmbeddingBags(
             embedding_specs=[(t.name, t.local_rows, t.local_cols, t.data_type) for t in config.embedding_tables],
             feature_table_map=[i for i, t in enumerate(config.embedding_tables) for _ in t.feature_names],
             pooling_mode=mode, output_dtype=out_dtype, device=dev, row_alignment=int((fused_params or {}).get("row_alignment", 16)),
+            locations=[loc for loc, _ in placement], cache_load_factor=[clf for _, clf in placement],
         )
         self._runtime_device = dev
 

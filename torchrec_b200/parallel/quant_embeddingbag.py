@@ -18,7 +18,7 @@ from ..quant.embedding_modules import EmbeddingBagCollection as QuantEmbeddingBa
 from ..quant.embedding_modules import EmbeddingCollection as QuantEmbeddingCollection
 from ..types import DataType
 from ..sparse.jagged_tensor import JaggedTensor, KeyedJaggedTensor, KeyedTensor
-from .embedding_types import BaseQuantEmbeddingSharder
+from .embedding_types import BaseQuantEmbeddingSharder, quant_table_placement
 from .engine import shards_of
 from .types import NullShardedModuleContext, ParameterSharding, ShardedModule, ShardingEnv, ShardingType, LazyNoWait, NoWait
 
@@ -75,15 +75,20 @@ class ShardedQuantEmbeddingBagCollection(ShardedModule[List[KeyedJaggedTensor], 
                 self._rank_meta.append([])
                 continue
             shard_keys: List[Tuple[int, int, int]] = []
-            specs = []
+            specs, locs, clfs = [], [], []
             for ti, s, fi in units:
                 key = (ti, s.row_off, s.col_off)
                 if key not in shard_keys:
                     shard_keys.append(key)
                     specs.append((f"{tables[ti].name}_{s.row_off}_{s.col_off}", s.rows, s.cols, tables[ti].data_type))
+                    ps = table_name_to_parameter_sharding[tables[ti].name]
+                    loc, clf = quant_table_placement(ps.compute_kernel, getattr(ps, "cache_params", None), fused_params)
+                    locs.append(loc)
+                    clfs.append(clf)
             fmap = [shard_keys.index((ti, s.row_off, s.col_off)) for ti, s, fi in units]
             pool = {tables[ti].pooling for ti, _, _ in units}
-            tbe = QuantTableBatchedEmbeddingBags(specs, fmap, pooling_mode=0, output_dtype=self._output_dtype, device=dev)
+            tbe = QuantTableBatchedEmbeddingBags(specs, fmap, pooling_mode=0, output_dtype=self._output_dtype, device=dev, locations=locs,
+                                                 cache_load_factor=clfs)
             # fill: dequantise the source slice and re-quantise the shard (column slices change the row scale)
             from ..ops.quant_tbe import dequantize_rows
 
@@ -336,6 +341,17 @@ class _InferencePlane:
                     def launch(f0: int, f1: int, out_ptr: int, out_stride: int) -> None:
                         if f1 <= f0:
                             return
+                        if tbe._placed:  # host-resident tables (and their HBM row caches) next to HBM tables in the same launch
+                            c = L.trb_qtbe_fwd_placed(
+                                ctypes.c_void_p(tbe.feat_base.data_ptr() + 8 * f0), ctypes.c_void_p(tbe.feat_ctab.data_ptr() + 4 * f0),
+                                _lib.ptr(tbe.cache_tabs), _lib.ptr(tbe.no_slot), ctypes.c_void_p(tbe.feat_rows.data_ptr() + 8 * f0),
+                                ctypes.c_void_p(tbe.feat_dim.data_ptr() + 4 * f0), ctypes.c_void_p(self.dev_direct[r].data_ptr() + 4 * f0),
+                                ctypes.c_void_p(tbe.feat_fmt.data_ptr() + 4 * f0), ctypes.c_void_p(tbe.feat_rb.data_ptr() + 4 * f0), _lib.ptr(self.val_bufs[r]),
+                                int(self.idx_dtype == torch.int64), ctypes.c_void_p(self.off_bufs[r].data_ptr() + 4 * f0 * B), 0, _lib.ptr(psw),
+                                ctypes.c_void_p(out_ptr), _lib.dtype_code(m._output_dtype), ctypes.c_int64(out_stride), B, f1 - f0, tbe.max_dim, 0, 1,
+                                ctypes.c_int64(0), int(tbe._uniform_fmt), _lib.stream_ptr(self.devs[r]))
+                            _lib.check(c, "trb_qtbe_fwd_placed")
+                            return
                         c = L.trb_qtbe_fwd_ex(
                             _lib.ptr(tbe.weights), ctypes.c_void_p(tbe.feat_woff.data_ptr() + 8 * f0), ctypes.c_void_p(tbe.feat_rows.data_ptr() + 8 * f0),
                             ctypes.c_void_p(tbe.feat_dim.data_ptr() + 4 * f0), ctypes.c_void_p(self.dev_direct[r].data_ptr() + 4 * f0),
@@ -345,9 +361,13 @@ class _InferencePlane:
                             _lib.stream_ptr(self.devs[r]))
                         _lib.check(c, "trb_qtbe_fwd_ex")
 
+                    if tbe._placed:
+                        tbe._wait_admission()
                     launch(0, n_direct, res.data_ptr(), m._total_cols)  # pooled rows -> final columns of the result on device 0 (peer stores)
                     if n_direct < F:
                         launch(n_direct, F, self.staging.data_ptr() + r * B * self.staged_width * esz, self.staged_width)
+                    if tbe._placed and tbe._cached:
+                        tbe._admit()  # this device's admission, on its side stream
                     if r != 0:
                         ev = torch.cuda.Event()
                         ev.record(st)

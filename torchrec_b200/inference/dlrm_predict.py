@@ -17,7 +17,7 @@ from ..models.dlrm import DLRM
 from ..modules.embedding_configs import DataType, EmbeddingBagConfig
 from ..modules.embedding_modules import EmbeddingBagCollection
 from ..sparse import KeyedJaggedTensor
-from .modules import BatchingMetadata, PredictFactory, PredictModule, quantize_inference_model, shard_quant_model
+from .modules import BatchingMetadata, PredictFactory, PredictModule, quantize_dense, quantize_inference_model, shard_quant_model
 
 logger: logging.Logger = logging.getLogger(__name__)
 
@@ -34,6 +34,9 @@ class DLRMModelConfig:
     sample_input: Optional[Batch] = None
     weight_dtype: DataType = DataType.INT8
     per_table_weight_dtype: Dict[str, DataType] = field(default_factory=dict)
+    # dtype of the dense arch (bottom / top MLP, cross net) in the served module: None keeps it as trained; torch.float8_e4m3fn runs it
+    # on the FP8 GEMM (quantize_dense)
+    dense_dtype: Optional[torch.dtype] = None
 
 
 def create_training_batch(num_dense: int, keys: List[str], num_embeddings: int, batch_size: int, ids_per_feature: int = 1, seed: int = 0) -> Batch:
@@ -109,6 +112,8 @@ class DLRMPredictFactory(PredictFactory):
         return quantize_inference_model(predict_module, quantization_dtype=cfg.weight_dtype, per_table_weight_dtype=per_table)
 
     def run_weights_dependent_transformations(self, predict_module: torch.nn.Module) -> torch.nn.Module:
+        if self.model_config.dense_dtype is not None:
+            predict_module = quantize_dense(predict_module, self.model_config.dense_dtype)
         return predict_module
 
     def model_inputs_data(self) -> Dict[str, object]:

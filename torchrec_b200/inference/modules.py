@@ -150,8 +150,27 @@ def quantize_embeddings(module: nn.Module, dtype: Union[torch.dtype, DataType], 
 
 
 def quantize_dense(predict_module: nn.Module, dtype: torch.dtype, additional_embedding_module_type: Optional[List[Type[nn.Module]]] = None) -> nn.Module:
-    """Cast the dense (non-embedding) parameters to ``dtype`` (fp16 / bf16 serving)."""
+    """Cast the dense (non-embedding) parameters to ``dtype`` (fp16 / bf16 serving).
+
+    ``dtype=torch.float8_e4m3fn`` instead swaps every ``MLP`` and ``LowRankCrossNet`` outside the embedding collections for its FP8
+    inference form (``quant.dense_modules``: ``Fp8MLP``, ``Fp8LowRankCrossNet``) and leaves every other parameter as it is. An MLP
+    without an FP8-eligible layer and a cross net whose width or rank is not a multiple of 16 stay unchanged."""
     skip = (EmbeddingBagCollectionInterface, EmbeddingCollectionInterface) + tuple(additional_embedding_module_type or [])
+    if dtype == torch.float8_e4m3fn:
+        from ..quant.dense_modules import Fp8LowRankCrossNet, Fp8MLP
+
+        def swap(m: nn.Module) -> nn.Module:
+            if isinstance(m, skip):
+                return m
+            if Fp8MLP.eligible(m):
+                return Fp8MLP.from_float(m)
+            if Fp8LowRankCrossNet.eligible(m):
+                return Fp8LowRankCrossNet.from_float(m)
+            for name, child in list(m.named_children()):
+                setattr(m, name, swap(child))
+            return m
+
+        return swap(predict_module)
 
     def cast(m: nn.Module) -> None:
         if isinstance(m, skip):

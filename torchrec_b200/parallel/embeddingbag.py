@@ -21,6 +21,7 @@ from torch.nn.parallel import DistributedDataParallel
 
 from ..modules.embedding_configs import BaseEmbeddingConfig, DataType, EmbeddingBagConfig, PoolingType, data_type_to_dtype
 from ..modules.embedding_modules import EmbeddingBagCollection, EmbeddingBagCollectionInterface, get_embedding_names_by_table
+from ..ops import vbe as V
 from ..ops.tbe import OptimType, PoolingMode, TableBatchedEmbeddingBags, WeightDecayMode
 from ..optim.fused import EmptyFusedOptimizer, FusedOptimizer, FusedOptimizerModule
 from ..optim.keyed import CombinedOptimizer, KeyedOptimizer
@@ -265,12 +266,17 @@ class EmbeddingBagCollectionContext(Multistreamable):
         self.inverse_indices: Optional[Tuple[List[str], torch.Tensor]] = None
         self.sharding_contexts: List[Any] = []
         self.B_local: int = 0
+        self.variable_batch_per_feature: bool = False
+        self.vbe_full: bool = False  # VBE batch padded to the width of its inverse indices: it takes the NVLink plane
+        self.vbe_index: Optional[V.VbeIndex] = None  # inverse indices + their CSR, read by the expansion and by its backward
 
     def record_stream(self, stream: torch.Stream) -> None:
         if self.mean_divisor is not None and self.mean_divisor.is_cuda:
             self.mean_divisor.record_stream(stream)
         if self.dp_features is not None:
             self.dp_features.record_stream(stream)
+        if self.vbe_index is not None:
+            self.vbe_index.record_stream(stream)
 
 
 class _InputDistAwaitable(Awaitable[Awaitable[KJTList]]):
@@ -427,6 +433,7 @@ class ShardedEmbeddingBagCollection(
         self._features_order: Optional[List[int]] = None
         self._has_features_permute = False
         self._optim: Optional[KeyedOptimizer] = None
+        self._vbe_col_tables: Dict[Tuple, Any] = {}  # static column -> inverse-row tables of VBE batches (ops/vbe.py), per inverse-key order
 
     # ---- construction helpers -----------------------------------------------------------------------------
     @torch.no_grad()
@@ -559,35 +566,38 @@ class ShardedEmbeddingBagCollection(
         self._features_order = order
         self._has_features_permute = order != list(range(len(keys)))
 
-    @staticmethod
-    def _pad_vbe(features: KeyedJaggedTensor) -> KeyedJaggedTensor:
-        """Variable batch per feature -> uniform stride max_f(B_f) by appending empty bags (values untouched)."""
+    def _plane_serves(self, B: int) -> bool:
+        """A uniform batch of ``B`` samples per feature takes the NVLink plane (fused input dist, lookup + output dist)."""
+        eng = self._engine
+        return eng is not None and not self._needs_dist_kjt and eng.fused_available(None) and eng._uniform_batch(B)
+
+    def _pad_vbe(self, ctx: EmbeddingBagCollectionContext, features: KeyedJaggedTensor) -> KeyedJaggedTensor:
+        """Variable batch per feature -> one stride by appending empty bags (values untouched). A device batch with inverse indices
+        ``[R, B]`` whose features all have ``B_f <= B`` is padded to ``B`` when the NVLink plane serves that stride: ``B`` is the same
+        every step, so the plane's buffers, its CUDA graphs and the uniform-batch check see one size (``ctx.vbe_full``). Any other
+        batch - and any batch the plane does not serve, whose bags travel through the routed input dist and the collective output
+        dist - is padded to ``max_f B_f`` only. The expansion index (CSR of the inverse indices, ids only) is built here, next to the
+        routing work, and kept in the context for the backward."""
+        inv = features.inverse_indices_or_none()
         spk = features.stride_per_key()
-        Bm = max(spk) if spk else 0
-        lengths = features.lengths()
-        padded = lengths.new_zeros(len(spk), Bm)
-        pos = 0
-        for f, b in enumerate(spk):
-            padded[f, :b] = lengths[pos : pos + b]
-            pos += b
-        return KeyedJaggedTensor(keys=features.keys(), values=features.values(), weights=features.weights_or_none(), lengths=padded.reshape(-1), stride=Bm)
+        stride = max(spk) if spk else 0
+        ctx.vbe_full = (inv is not None and features.values().is_cuda and inv[1].is_cuda and stride <= inv[1].shape[1]
+                        and self._plane_serves(inv[1].shape[1]))
+        if ctx.vbe_full:
+            stride = inv[1].shape[1]
+        padded = V.pad_offsets(features, stride)
+        if inv is not None:
+            ctx.vbe_index = V.VbeIndex(inv, self._embedding_names, self._embedding_dims, src_rows=stride, tables=self._vbe_col_tables)
+            if ctx.vbe_full and torch.is_grad_enabled():
+                ctx.vbe_index.csr()
+        return padded
 
     def _vbe_expand(self, ctx: EmbeddingBagCollectionContext, kt: KeyedTensor) -> KeyedTensor:
-        """Undo the de-duplication of a VBE batch: out[b, cols(f)] = pooled[inverse_indices[f, b], cols(f)]
-        (reference embeddingbag.py:405 / VariableBatchPooledEmbeddingsAllToAll semantics)."""
-        inv = ctx.inverse_indices
-        if inv is None:
+        """Undo the de-duplication of a VBE batch: out[b, cols(f)] = pooled[inverse_indices[f, b], cols(f)]."""
+        index = ctx.vbe_index
+        if index is None:
             return kt
-        keys, idx = inv
-        row = {k: i for i, k in enumerate(keys)}
-        vals = kt.values()
-        outs = []
-        c = 0
-        for name, d in zip(self._embedding_names, self._embedding_dims):
-            feat = name.split("@")[0]
-            outs.append(vals[:, c : c + d].index_select(0, idx[row[feat]].long()) if feat in row else vals[:, c : c + d])
-            c += d
-        return KeyedTensor(keys=kt.keys(), length_per_key=kt.length_per_key(), values=torch.cat(outs, dim=1), key_dim=1)
+        return KeyedTensor(keys=kt.keys(), length_per_key=kt.length_per_key(), values=V.vbe_expand(kt.values(), index), key_dim=1)
 
     def input_dist(self, ctx: EmbeddingBagCollectionContext, features: KeyedJaggedTensor) -> Awaitable[Awaitable[KJTList]]:
         if self._features_order is None:
@@ -596,11 +606,10 @@ class ShardedEmbeddingBagCollection(
             # VBE: ship the de-duplicated bags (padded to one stride), expand with inverse_indices after the output dist
             ctx.inverse_indices = features.inverse_indices_or_none()
             ctx.variable_batch_per_feature = True
-            features = self._pad_vbe(features)
+            features = self._pad_vbe(ctx, features)
         with torch.no_grad():
             eng = self._engine
-            if (eng is not None and not getattr(ctx, "variable_batch_per_feature", False) and not self._needs_dist_kjt and eng.fused_available(None)
-                    and eng._uniform_batch(features.stride())):
+            if ctx.vbe_full or (not ctx.variable_batch_per_feature and self._plane_serves(features.stride())):
                 # NVLink plane: bucketize + feature permute + peer write in one device-side pass, straight from the batch's KJT
                 # (any mix of sharding types); the only host work is picking the slot
                 order = self._features_order
@@ -682,7 +691,7 @@ class ShardedEmbeddingBagCollection(
             eng = self._engine if self._engine is not None else _COMBINE_ONLY
             vals = eng.combine(mp, dp_out, self._dp_cols, self._total_cols, ctx.mean_divisor)
             kt = KeyedTensor(keys=self._embedding_names, length_per_key=self._embedding_dims, values=vals, key_dim=1)
-            return self._vbe_expand(ctx, kt) if getattr(ctx, "variable_batch_per_feature", False) else kt
+            return self._vbe_expand(ctx, kt) if ctx.variable_batch_per_feature else kt
 
         return EmbeddingBagCollectionAwaitable(finish)
 
@@ -714,7 +723,7 @@ class ShardedEmbeddingBagCollection(
         if ctx.mean_divisor is not None:
             vals = vals * ctx.mean_divisor.to(vals.dtype)
         kt = KeyedTensor(keys=self._embedding_names, length_per_key=self._embedding_dims, values=vals, key_dim=1)
-        if getattr(ctx, "variable_batch_per_feature", False):
+        if ctx.variable_batch_per_feature:
             kt = self._vbe_expand(ctx, kt)
         return EmbeddingBagCollectionAwaitable(lambda: kt)
 

@@ -6,6 +6,7 @@
 // load/store them directly over NVSwitch.
 // NCCL stays the control plane (handle exchange, DDP all-reduce, multi-node fallback).
 #include "common.cuh"
+#include "qcomm_fp8.cuh"
 #include <cstring>
 #include <cstdio>
 
@@ -315,4 +316,124 @@ TRB_API int trb_grad_push(const void* src, int s_dtype, int64_t src_stride, cons
   TRB_GP(TRB_BF16, __nv_bfloat16, TRB_BF16, __nv_bfloat16)
 #undef TRB_GP
   return -3;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// FP8 wire of the sparse plane (format: qcomm_fp8.cuh). The push quantizes each gradient chunk of R = row_dim columns on the
+// source and stores e4m3 payload + one fp32 scale into the owner's FP8 inbox; after the barrier `trb_fp8_wire_decode` turns
+// payload + scales back into wire-dtype rows (the gradient inbox, or the pooled output of the forward).
+// ---------------------------------------------------------------------------------------------------------------
+// L = row_dim / 8 lanes per chunk, 8 values per lane; the lanes of a chunk are adjacent and aligned inside a warp, and since the
+// work count is a multiple of L they enter and leave the grid-stride loop together (the amax shuffle needs all of them).
+template <typename S, int UNR>
+__global__ void __launch_bounds__(256)
+trb_grad_push_fp8_kernel(const S* __restrict__ src, int64_t src_stride, const int32_t* __restrict__ chunks, int n_chunks, TrbPeerPtrs dst,
+                         TrbPeerPtrs dst_scale, int64_t dst_pitch, int64_t scale_pitch, int64_t row_base, int B_local, int L) {
+  const int64_t total = (int64_t) B_local * n_chunks * L;
+  const int64_t stride = (int64_t) gridDim.x * blockDim.x;
+  const int lane = threadIdx.x & 31;
+  const unsigned gmask = L == 32 ? 0xffffffffu : ((1u << L) - 1u) << (lane & ~(L - 1));
+  const int lig = lane & (L - 1);
+  for (int64_t i0 = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; i0 < total; i0 += stride * UNR) {
+    float4 v[UNR][2];
+    int64_t row[UNR];
+    int rank[UNR], dc[UNR];
+    bool ok[UNR];
+#pragma unroll
+    for (int u = 0; u < UNR; ++u) {
+      const int64_t i = i0 + u * stride;
+      ok[u] = i < total;
+      const int64_t item = (ok[u] ? i : i0) / L;
+      const int64_t b = item / n_chunks;
+      const int c = (int) (item - b * n_chunks);
+      rank[u] = chunks[3 * c];
+      dc[u] = chunks[3 * c + 2];
+      row[u] = row_base + b;
+      const S* sp = src + b * src_stride + chunks[3 * c + 1] + lig * 8;
+      v[u][0] = Vec4<S>::ld(sp);
+      v[u][1] = Vec4<S>::ld(sp + 4);
+    }
+#pragma unroll
+    for (int u = 0; u < UNR; ++u) {
+      float amax = fmaxf(trb_fp8_abs_max4(v[u][0]), trb_fp8_abs_max4(v[u][1]));
+      for (int o = L >> 1; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(gmask, amax, o));
+      if (!ok[u]) continue;
+      const float scale = trb_fp8_scale(amax);
+      const float inv = 1.f / scale;
+      uint8_t* q = reinterpret_cast<uint8_t*>(dst.p[rank[u]]) + row[u] * dst_pitch + dc[u] + lig * 8;
+      *reinterpret_cast<uint2*>(q) = make_uint2(trb_fp8_encode4(v[u][0], inv), trb_fp8_encode4(v[u][1], inv));
+      if (lig == 0) reinterpret_cast<float*>(dst_scale.p[rank[u]])[row[u] * scale_pitch + dc[u] / (8 * L)] = scale;
+    }
+  }
+}
+
+// chunks: int32 [n_chunks, 3] (destination rank, source column, inbox column), each `row_dim` (32 | 64 | 128) columns wide.
+// dst_ptrs / scale_ptrs: every rank's uint8 payload inbox [*, dst_pitch] and fp32 scale inbox [*, scale_pitch]; source row b lands
+// in row row_base + b.
+TRB_API int trb_grad_push_fp8(const void* src, int s_dtype, int64_t src_stride, const int32_t* chunks, int n_chunks, int row_dim, void* const* dst_ptrs,
+                              void* const* scale_ptrs, int n_dst, int64_t dst_pitch, int64_t scale_pitch, int64_t row_base, int B_local, cudaStream_t stream) {
+  if (n_dst < 1 || n_dst > TRB_MAX_PEERS || (row_dim != 32 && row_dim != 64 && row_dim != 128)) return -1;
+  const int L = row_dim / 8;
+  const int64_t n = (int64_t) B_local * n_chunks * L;
+  if (n == 0) return 0;
+  TrbPeerPtrs d, ds;
+  for (int i = 0; i < n_dst; ++i) {
+    d.p[i] = dst_ptrs[i];
+    ds.p[i] = scale_ptrs[i];
+  }
+  const int threads = 256;
+  constexpr int UNR = 4;
+  constexpr int kPushCtasPerSm = 2;  // as trb_grad_push: leaves room for the GEMMs that run beside the push
+  const int sms = trb_num_sms();
+  const int64_t want = (n + (int64_t) threads * UNR - 1) / ((int64_t) threads * UNR);
+  const unsigned blocks = (unsigned) (want < (int64_t) sms * kPushCtasPerSm ? want : (int64_t) sms * kPushCtasPerSm);
+  if (s_dtype == TRB_F32) {
+    trb_grad_push_fp8_kernel<float, UNR><<<blocks, threads, 0, stream>>>((const float*) src, src_stride, chunks, n_chunks, d, ds, dst_pitch, scale_pitch, row_base, B_local, L);
+  } else if (s_dtype == TRB_BF16) {
+    trb_grad_push_fp8_kernel<__nv_bfloat16, UNR><<<blocks, threads, 0, stream>>>((const __nv_bfloat16*) src, src_stride, chunks, n_chunks, d, ds, dst_pitch, scale_pitch,
+                                                                                 row_base, B_local, L);
+  } else {
+    return -3;
+  }
+  TRB_CHECK_LAUNCH();
+  return 0;
+}
+
+// out[r, c : c + 16] = decode(payload[r, c : c + 16], scales[r, c / row_dim]) stored as O, for every row r < rows and every 16-column
+// chunk start c in `cols` (a static list: the FP8 columns only, other columns of `out` are left alone). One 16-byte load per thread.
+template <typename O>
+__global__ void __launch_bounds__(256)
+trb_fp8_wire_decode_kernel(const uint8_t* __restrict__ pay, int64_t pay_pitch, const float* __restrict__ scales, int64_t scale_pitch, int row_dim,
+                           const int32_t* __restrict__ cols, int n_cols, int64_t rows, O* __restrict__ out, int64_t out_pitch) {
+  const int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= rows * n_cols) return;
+  const int64_t r = i / n_cols;
+  const int c = cols[i - r * n_cols];
+  const uint4 q = *reinterpret_cast<const uint4*>(pay + r * pay_pitch + c);
+  const float s = scales[r * scale_pitch + c / row_dim];
+  O* o = out + r * out_pitch + c;
+  Vec4<O>::st(o, trb_fp8_decode4(q.x, s));
+  Vec4<O>::st(o + 4, trb_fp8_decode4(q.y, s));
+  Vec4<O>::st(o + 8, trb_fp8_decode4(q.z, s));
+  Vec4<O>::st(o + 12, trb_fp8_decode4(q.w, s));
+}
+
+TRB_API int trb_fp8_wire_decode(const void* payload, int64_t pay_pitch, const float* scales, int64_t scale_pitch, int row_dim, const int32_t* cols, int n_cols,
+                                int64_t rows, void* out, int out_dtype, int64_t out_pitch, cudaStream_t stream) {
+  if (row_dim % 16 != 0 || pay_pitch % 16 != 0) return -1;
+  const int64_t n = rows * n_cols;
+  if (n == 0) return 0;
+  const int threads = 256;
+  const unsigned blocks = (unsigned) ((n + threads - 1) / threads);
+  if (out_dtype == TRB_F32) {
+    trb_fp8_wire_decode_kernel<float><<<blocks, threads, 0, stream>>>((const uint8_t*) payload, pay_pitch, scales, scale_pitch, row_dim, cols, n_cols, rows,
+                                                                     (float*) out, out_pitch);
+  } else if (out_dtype == TRB_BF16) {
+    trb_fp8_wire_decode_kernel<__nv_bfloat16><<<blocks, threads, 0, stream>>>((const uint8_t*) payload, pay_pitch, scales, scale_pitch, row_dim, cols, n_cols,
+                                                                             rows, (__nv_bfloat16*) out, out_pitch);
+  } else {
+    return -3;
+  }
+  TRB_CHECK_LAUNCH();
+  return 0;
 }

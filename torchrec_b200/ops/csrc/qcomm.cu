@@ -8,7 +8,7 @@
 // One warp per row (FP8 / INT8) or per 32-element group (MX4, one lane per element); amax / min / max through shuffles; encode and
 // decode are single passes over the data. fp16 / bf16 codecs are plain casts (torch).
 #include "common.cuh"
-#include <cuda_fp8.h>
+#include "qcomm_fp8.cuh"
 
 __device__ __forceinline__ float warp_max(float v) {
 #pragma unroll
@@ -30,13 +30,10 @@ __global__ void __launch_bounds__(256) qcomm_fp8_encode_kernel(const float* __re
   float amax = 0.f;
   for (int i = lane; i < row_dim; i += 32) amax = fmaxf(amax, fabsf(src[i]));
   amax = warp_max(amax);
-  const float scale = amax > 0.f ? amax / 448.f : 1.f;
+  const float scale = trb_fp8_scale(amax);
   const float inv = 1.f / scale;
   uint8_t* dst = out + r * (int64_t) (row_dim + 4);
-  for (int i = lane; i < row_dim; i += 32) {
-    const __nv_fp8_e4m3 q(src[i] * inv);
-    dst[i] = *reinterpret_cast<const uint8_t*>(&q);
-  }
+  for (int i = lane; i < row_dim; i += 32) dst[i] = trb_fp8_encode(src[i], inv);
   if (lane == 0) memcpy(dst + row_dim, &scale, 4);
 }
 
@@ -48,11 +45,7 @@ __global__ void __launch_bounds__(256) qcomm_fp8_decode_kernel(const uint8_t* __
   float scale;
   memcpy(&scale, src + row_dim, 4);
   float* dst = out + r * row_dim;
-  for (int i = lane; i < row_dim; i += 32) {
-    __nv_fp8_e4m3 q;
-    *reinterpret_cast<uint8_t*>(&q) = src[i];
-    dst[i] = static_cast<float>(q) * scale;
-  }
+  for (int i = lane; i < row_dim; i += 32) dst[i] = trb_fp8_decode(src[i], scale);
 }
 
 // ---- INT8 row-wise (scale + bias) ----------------------------------------------------------------------------------------------------

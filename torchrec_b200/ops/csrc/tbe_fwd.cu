@@ -17,7 +17,12 @@
 //
 // Parity: replaces fbgemm SplitTableBatchedEmbeddingBagsCodegen forward
 // (reference call site torchrec/distributed/batched_embedding_kernel.py:3010-3058).
+//
+// FP8 wire (trb_tbe_pooled_fwd_fp8, instances with Q = true): the pooled row, rounded to the wire dtype O, is stored as
+// e4m3 groups of R = 4 * q_lanes columns plus one fp32 scale per group (qcomm_fp8.cuh). The R / 4 lanes that hold a group's
+// float4 vectors take its amax with a shuffle; there is no extra pass over the pooled rows.
 #include "common.cuh"
+#include "qcomm_fp8.cuh"
 
 unsigned long long g_trb_launches = 0;
 TRB_API unsigned long long trb_launch_count() { return g_trb_launches; }
@@ -38,8 +43,40 @@ struct TbeFwdParams {
   int32_t mean;                  // 1 = MEAN pooling
 };
 
-template <typename W, typename O, int LPB, int MAXV>
-__global__ void __launch_bounds__(256) tbe_pooled_fwd_kernel(const TbeFwdParams p) {
+// FP8 wire (Q = true instances only, so the other instances keep their parameter block): `out` points at uint8 payload rows,
+// `q_scale` at fp32 rows of one scale per group of 4 * q_lanes columns
+struct TbeFwdQParams : TbeFwdParams {
+  TrbPeerPtrs q_scale;
+  int64_t q_scale_stride;
+  int32_t q_lanes;
+};
+
+template <bool Q>
+struct TbeFwdParamsOf {
+  using type = TbeFwdParams;
+};
+template <>
+struct TbeFwdParamsOf<true> {
+  using type = TbeFwdQParams;
+};
+
+// FP8 store of the 4 values of output columns [c, c + 4) of row `bl` of destination `s`. Every lane of the q_lanes-lane group
+// that holds the R columns must call it (`ok` false for lanes past the row): the group amax is a shuffle across them.
+template <typename O>
+__device__ __forceinline__ void fp8_wire_store(const TbeFwdQParams& p, int s, int bl, int c, float4 v, bool ok, unsigned mask) {
+  v = trb_round_to<O>(v);
+  float amax = ok ? trb_fp8_abs_max4(v) : 0.f;
+  for (int o = p.q_lanes >> 1; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(mask, amax, o));
+  if (!ok) return;
+  const float scale = trb_fp8_scale(amax);
+  uint8_t* q = reinterpret_cast<uint8_t*>(p.out.p[s]) + (int64_t) bl * p.out_stride + c;
+  *reinterpret_cast<uint32_t*>(q) = trb_fp8_encode4(v, 1.f / scale);
+  const int R = p.q_lanes * 4;
+  if (c % R == 0) reinterpret_cast<float*>(p.q_scale.p[s])[(int64_t) bl * p.q_scale_stride + c / R] = scale;
+}
+
+template <typename W, typename O, int LPB, int MAXV, bool Q = false>
+__global__ void __launch_bounds__(256) tbe_pooled_fwd_kernel(const typename TbeFwdParamsOf<Q>::type p) {
   constexpr int UNROLL = (MAXV <= 2) ? 4 : (MAXV <= 4 ? 2 : 1);
   const int lig = threadIdx.x % LPB;  // lane in group
   const int64_t group = ((int64_t) blockIdx.x * blockDim.x + threadIdx.x) / LPB;
@@ -101,11 +138,20 @@ __global__ void __launch_bounds__(256) tbe_pooled_fwd_kernel(const TbeFwdParams 
   }
   const int s = b / p.B_local;
   const int bl = b - s * p.B_local;
-  O* dst = reinterpret_cast<O*>(p.out.p[s]) + (int64_t) bl * p.out_stride + p.feat_col[f];
+  if constexpr (Q) {
+    const int col = p.feat_col[f];
 #pragma unroll
-  for (int k = 0; k < MAXV; ++k) {
-    const int vi = lig + k * LPB;
-    if (vi < nvec) Vec4<O>::st(dst + vi * 4, acc[k]);
+    for (int k = 0; k < MAXV; ++k) {
+      const int vi = lig + k * LPB;
+      fp8_wire_store<O>(p, s, bl, col + vi * 4, acc[k], vi < nvec, gmask);
+    }
+  } else {
+    O* dst = reinterpret_cast<O*>(p.out.p[s]) + (int64_t) bl * p.out_stride + p.feat_col[f];
+#pragma unroll
+    for (int k = 0; k < MAXV; ++k) {
+      const int vi = lig + k * LPB;
+      if (vi < nvec) Vec4<O>::st(dst + vi * 4, acc[k]);
+    }
   }
 }
 
@@ -115,8 +161,8 @@ __global__ void __launch_bounds__(256) tbe_pooled_fwd_kernel(const TbeFwdParams 
 // ids are issued back to back (U independent 512 B requests in flight per warp) before any of
 // them is consumed — with one id per bag (Criteo) this is what hides the HBM latency.
 // ------------------------------------------------------------------------------------------------
-template <typename W, typename O, int MAXV, int U>
-__global__ void __launch_bounds__(256) tbe_pooled_fwd_chunk_kernel(const TbeFwdParams p) {
+template <typename W, typename O, int MAXV, int U, bool Q = false>
+__global__ void __launch_bounds__(256) tbe_pooled_fwd_chunk_kernel(const typename TbeFwdParamsOf<Q>::type p) {
   const int lane = threadIdx.x & 31;
   const int64_t chunk = ((int64_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   // chunks never straddle a source region or a destination: they tile the finer of the two partitions of the batch
@@ -179,11 +225,19 @@ __global__ void __launch_bounds__(256) tbe_pooled_fwd_chunk_kernel(const TbeFwdP
         for (int u = 0; u < U; ++u) {
           if (j + u < nb) {
             const float w = __shfl_sync(0xffffffffu, my_w, j + u);
-            O* dst = dst0 + (int64_t) (j + u) * p.out_stride;
+            if constexpr (Q) {
 #pragma unroll
-            for (int k = 0; k < MAXV; ++k) {
-              const int vi = lane + k * 32;
-              if (vi < nvec) Vec4<O>::st(dst + vi * 4, f4_scale(v[u][k], w));
+              for (int k = 0; k < MAXV; ++k) {
+                const int vi = lane + k * 32;
+                fp8_wire_store<O>(p, s0, b0 - s0 * p.B_local + j + u, col + vi * 4, f4_scale(v[u][k], w), vi < nvec, 0xffffffffu);
+              }
+            } else {
+              O* dst = dst0 + (int64_t) (j + u) * p.out_stride;
+#pragma unroll
+              for (int k = 0; k < MAXV; ++k) {
+                const int vi = lane + k * 32;
+                if (vi < nvec) Vec4<O>::st(dst + vi * 4, f4_scale(v[u][k], w));
+              }
             }
           }
         }
@@ -208,12 +262,21 @@ __global__ void __launch_bounds__(256) tbe_pooled_fwd_chunk_kernel(const TbeFwdP
     const int b = b0 + bag_in_chunk;
     const int s = b / p.B_local;
     const int bl = b - s * p.B_local;
-    O* dst = reinterpret_cast<O*>(p.out.p[s]) + (int64_t) bl * p.out_stride + col;
+    if constexpr (Q) {
 #pragma unroll
-    for (int k = 0; k < MAXV; ++k) {
-      const int vi = lane + k * 32;
-      if (vi < nvec) Vec4<O>::st(dst + vi * 4, acc[k]);
-      acc[k] = make_float4(0.f, 0.f, 0.f, 0.f);
+      for (int k = 0; k < MAXV; ++k) {
+        const int vi = lane + k * 32;
+        fp8_wire_store<O>(p, s, bl, col + vi * 4, acc[k], vi < nvec, 0xffffffffu);
+        acc[k] = make_float4(0.f, 0.f, 0.f, 0.f);
+      }
+    } else {
+      O* dst = reinterpret_cast<O*>(p.out.p[s]) + (int64_t) bl * p.out_stride + col;
+#pragma unroll
+      for (int k = 0; k < MAXV; ++k) {
+        const int vi = lane + k * 32;
+        if (vi < nvec) Vec4<O>::st(dst + vi * 4, acc[k]);
+        acc[k] = make_float4(0.f, 0.f, 0.f, 0.f);
+      }
     }
   };
 
@@ -266,64 +329,63 @@ __global__ void __launch_bounds__(256) tbe_pooled_fwd_chunk_kernel(const TbeFwdP
   }
 }
 
-template <typename W, typename O, int MAXV, int U>
-static int launch_pooled_chunk(const TbeFwdParams& p, cudaStream_t stream) {
+template <typename W, typename O, int MAXV, int U, bool Q>
+static int launch_pooled_chunk(const typename TbeFwdParamsOf<Q>::type& p, cudaStream_t stream) {
   if (p.B == 0 || p.F == 0) return 0;
   const int part = p.src.src_B < p.B_local ? p.src.src_B : p.B_local;
   const int64_t chunks = (int64_t) p.F * ((part + 31) / 32) * (p.B / part);
   if (chunks == 0) return 0;
   const int threads = 256;
   const int64_t blocks = (chunks + 7) / 8;
-  tbe_pooled_fwd_chunk_kernel<W, O, MAXV, U><<<(unsigned) blocks, threads, 0, stream>>>(p);
+  tbe_pooled_fwd_chunk_kernel<W, O, MAXV, U, Q><<<(unsigned) blocks, threads, 0, stream>>>(p);
   TRB_CHECK_LAUNCH();
   return 0;
 }
 
-template <typename W, typename O, int LPB, int MAXV>
-static int launch_pooled(const TbeFwdParams& p, cudaStream_t stream) {
+template <typename W, typename O, int LPB, int MAXV, bool Q>
+static int launch_pooled(const typename TbeFwdParamsOf<Q>::type& p, cudaStream_t stream) {
   const int64_t n_bags = (int64_t) p.F * p.B;
   if (n_bags == 0) return 0;
   const int threads = 256;
   const int64_t groups_per_block = threads / LPB;
   const int64_t blocks = (n_bags + groups_per_block - 1) / groups_per_block;
-  tbe_pooled_fwd_kernel<W, O, LPB, MAXV><<<(unsigned) blocks, threads, 0, stream>>>(p);
+  tbe_pooled_fwd_kernel<W, O, LPB, MAXV, Q><<<(unsigned) blocks, threads, 0, stream>>>(p);
   TRB_CHECK_LAUNCH();
   return 0;
 }
 
-template <typename W, typename O>
-static int dispatch_shape(const TbeFwdParams& p, int max_dim, cudaStream_t stream) {
+template <typename W, typename O, bool Q = false>
+static int dispatch_shape(const typename TbeFwdParamsOf<Q>::type& p, int max_dim, cudaStream_t stream) {
   const int nvec = max_dim / 4;
-  if (nvec <= 8) return launch_pooled<W, O, 8, 1>(p, stream);
-  if (nvec <= 16) return launch_pooled<W, O, 16, 1>(p, stream);
-  if (nvec <= 32) return launch_pooled_chunk<W, O, 1, 8>(p, stream);
-  if (nvec <= 64) return launch_pooled_chunk<W, O, 2, 4>(p, stream);
-  if (nvec <= 128) return launch_pooled_chunk<W, O, 4, 2>(p, stream);
-  if (nvec <= 512) return launch_pooled<W, O, 32, 16>(p, stream);
+  if constexpr (Q) {
+    if (p.q_lanes > (nvec <= 8 ? 8 : nvec <= 16 ? 16 : 32)) return -5;  // an FP8 group must lie inside the lanes of one row
+  }
+  if (nvec <= 8) return launch_pooled<W, O, 8, 1, Q>(p, stream);
+  if (nvec <= 16) return launch_pooled<W, O, 16, 1, Q>(p, stream);
+  if (nvec <= 32) return launch_pooled_chunk<W, O, 1, 8, Q>(p, stream);
+  if (nvec <= 64) return launch_pooled_chunk<W, O, 2, 4, Q>(p, stream);
+  if (nvec <= 128) return launch_pooled_chunk<W, O, 4, 2, Q>(p, stream);
+  if (nvec <= 512) return launch_pooled<W, O, 32, 16, Q>(p, stream);
   return -2;  // dim > 2048 unsupported
 }
 
-template <typename W>
-static int dispatch_out(const TbeFwdParams& p, int out_dtype, int max_dim, cudaStream_t stream) {
+template <typename W, bool Q = false>
+static int dispatch_out(const typename TbeFwdParamsOf<Q>::type& p, int out_dtype, int max_dim, cudaStream_t stream) {
   switch (out_dtype) {
-    case TRB_F32: return dispatch_shape<W, float>(p, max_dim, stream);
-    case TRB_BF16: return dispatch_shape<W, __nv_bfloat16>(p, max_dim, stream);
+    case TRB_F32: return dispatch_shape<W, float, Q>(p, max_dim, stream);
+    case TRB_BF16: return dispatch_shape<W, __nv_bfloat16, Q>(p, max_dim, stream);
   }
   return -3;
 }
 
-// Pooled forward. Returns 0 on success, a cudaError_t (>0) or a negative library error.
-// `n_src` > 1: ids arrive in per-source regions (see TrbSrcView); idx_stride / off_stride in elements.
-TRB_API int trb_tbe_pooled_fwd(const void* weights, int w_dtype, const int64_t* feat_woff, const int64_t* feat_rows,
-                               const int32_t* feat_dim, const int32_t* feat_col, const void* indices, int idx64,
-                               const void* offsets, int off64, const float* psw, int n_src, int64_t idx_stride, int64_t off_stride,
-                               void* const* out_ptrs, int n_out, int out_dtype, int64_t out_stride, int B, int B_local, int F,
-                               int max_dim, int mean, cudaStream_t stream) {
+static int pooled_fwd_params(TbeFwdParams& p, const void* weights, const int64_t* feat_woff, const int64_t* feat_rows, const int32_t* feat_dim,
+                             const int32_t* feat_col, const void* indices, int idx64, const void* offsets, int off64, const float* psw, int n_src,
+                             int64_t idx_stride, int64_t off_stride, void* const* out_ptrs, int n_out, int64_t out_stride, int B, int B_local, int F,
+                             int mean) {
   if (n_out < 1 || n_out > TRB_MAX_PEERS) return -1;
   if ((int64_t) B_local * n_out != B) return -4;
   if (n_src < 1 || B % n_src != 0) return -4;
   if (n_src > 1 && n_out > 1 && n_src != n_out) return -4;
-  TbeFwdParams p;
   p.weights = weights;
   p.feat_woff = feat_woff;
   p.feat_rows = feat_rows;
@@ -344,10 +406,48 @@ TRB_API int trb_tbe_pooled_fwd(const void* weights, int w_dtype, const int64_t* 
   p.B_local = B_local;
   p.F = F;
   p.mean = mean;
+  return 0;
+}
+
+// Pooled forward. Returns 0 on success, a cudaError_t (>0) or a negative library error.
+// `n_src` > 1: ids arrive in per-source regions (see TrbSrcView); idx_stride / off_stride in elements.
+TRB_API int trb_tbe_pooled_fwd(const void* weights, int w_dtype, const int64_t* feat_woff, const int64_t* feat_rows,
+                               const int32_t* feat_dim, const int32_t* feat_col, const void* indices, int idx64,
+                               const void* offsets, int off64, const float* psw, int n_src, int64_t idx_stride, int64_t off_stride,
+                               void* const* out_ptrs, int n_out, int out_dtype, int64_t out_stride, int B, int B_local, int F,
+                               int max_dim, int mean, cudaStream_t stream) {
+  TbeFwdParams p;
+  const int e = pooled_fwd_params(p, weights, feat_woff, feat_rows, feat_dim, feat_col, indices, idx64, offsets, off64, psw, n_src, idx_stride, off_stride,
+                                  out_ptrs, n_out, out_stride, B, B_local, F, mean);
+  if (e != 0) return e;
   switch (w_dtype) {
     case TRB_F32: return dispatch_out<float>(p, out_dtype, max_dim, stream);
     case TRB_F16: return dispatch_out<__half>(p, out_dtype, max_dim, stream);
     case TRB_BF16: return dispatch_out<__nv_bfloat16>(p, out_dtype, max_dim, stream);
+  }
+  return -3;
+}
+
+// Pooled forward with the FP8 wire: `out_ptrs` are uint8 payload rows [B_local, out_stride] per destination, `scale_ptrs` fp32
+// rows [B_local, scale_stride] per destination, one scale per `row_dim` columns (32, 64 or 128). Every feature's output column
+// and width must be multiples of row_dim. The groups are formed from the pooled values rounded to `wire_dtype` (fp32 | bf16).
+TRB_API int trb_tbe_pooled_fwd_fp8(const void* weights, int w_dtype, const int64_t* feat_woff, const int64_t* feat_rows,
+                                   const int32_t* feat_dim, const int32_t* feat_col, const void* indices, int idx64,
+                                   const void* offsets, int off64, const float* psw, int n_src, int64_t idx_stride, int64_t off_stride,
+                                   void* const* out_ptrs, void* const* scale_ptrs, int n_out, int wire_dtype, int64_t out_stride,
+                                   int64_t scale_stride, int row_dim, int B, int B_local, int F, int max_dim, int mean, cudaStream_t stream) {
+  if (row_dim != 32 && row_dim != 64 && row_dim != 128) return -5;
+  TbeFwdQParams p;
+  const int e = pooled_fwd_params(p, weights, feat_woff, feat_rows, feat_dim, feat_col, indices, idx64, offsets, off64, psw, n_src, idx_stride, off_stride,
+                                  out_ptrs, n_out, out_stride, B, B_local, F, mean);
+  if (e != 0) return e;
+  for (int i = 0; i < TRB_MAX_PEERS; ++i) p.q_scale.p[i] = i < n_out ? scale_ptrs[i] : nullptr;
+  p.q_scale_stride = scale_stride;
+  p.q_lanes = row_dim / 4;
+  switch (w_dtype) {
+    case TRB_F32: return dispatch_out<float, true>(p, wire_dtype, max_dim, stream);
+    case TRB_F16: return dispatch_out<__half, true>(p, wire_dtype, max_dim, stream);
+    case TRB_BF16: return dispatch_out<__nv_bfloat16, true>(p, wire_dtype, max_dim, stream);
   }
   return -3;
 }

@@ -537,10 +537,22 @@ class IdRegions:
 
 
 def pooled_forward_regions(meta: TbeMeta, weights: torch.Tensor, ids: IdRegions, mean: bool, out_dtype: torch.dtype, out_ptrs: Sequence[int],
-                           out_stride: int, B_local: int, device: torch.device) -> None:
-    """Pooled lookup over per-source id regions, pooled rows stored into ``out_ptrs`` (one buffer per destination rank)."""
+                           out_stride: int, B_local: int, device: torch.device, fp8: Optional[Tuple[Sequence[int], int, int]] = None) -> None:
+    """Pooled lookup over per-source id regions, pooled rows stored into ``out_ptrs`` (one buffer per destination rank).
+    ``fp8 = (scale_ptrs, scale_stride, row_dim)``: FP8 wire (csrc/qcomm_fp8.cuh) - ``out_ptrs`` are uint8 payload rows of ``out_stride``
+    bytes, ``scale_ptrs`` fp32 rows of ``scale_stride`` scales; the groups are formed from the rows rounded to ``out_dtype``."""
     L = _lib.lib()
     B = ids.n_src * ids.src_B
+    if fp8 is not None:
+        scale_ptrs, scale_stride, row_dim = fp8
+        code = L.trb_tbe_pooled_fwd_fp8(
+            _lib.ptr(weights), _lib.dtype_code(weights.dtype), _lib.ptr(meta.feat_woff), _lib.ptr(meta.feat_rows), _lib.ptr(meta.feat_dim), _lib.ptr(meta.feat_col),
+            ctypes.c_void_p(ids.idx_ptr), ids.idx64, ctypes.c_void_p(ids.off_ptr), ids.off64, ctypes.c_void_p(ids.psw_ptr), ids.n_src,
+            ctypes.c_int64(ids.idx_stride), ctypes.c_int64(ids.off_stride), _lib.ptr_array(out_ptrs), _lib.ptr_array(scale_ptrs), len(out_ptrs),
+            _lib.dtype_code(out_dtype), ctypes.c_int64(out_stride), ctypes.c_int64(scale_stride), int(row_dim), B, B_local, meta.num_features, meta.max_dim,
+            int(mean), _lib.stream_ptr(device))
+        _lib.check(code, "trb_tbe_pooled_fwd_fp8")
+        return
     code = L.trb_tbe_pooled_fwd(
         _lib.ptr(weights), _lib.dtype_code(weights.dtype), _lib.ptr(meta.feat_woff), _lib.ptr(meta.feat_rows), _lib.ptr(meta.feat_dim), _lib.ptr(meta.feat_col),
         ctypes.c_void_p(ids.idx_ptr), ids.idx64, ctypes.c_void_p(ids.off_ptr), ids.off64, ctypes.c_void_p(ids.psw_ptr), ids.n_src,

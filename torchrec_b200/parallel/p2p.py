@@ -166,3 +166,25 @@ def grad_push(src: torch.Tensor, chunks: torch.Tensor, dst_ptrs: List[int], dst_
     code = L.trb_grad_push(_lib.ptr(src), _lib.dtype_code(src.dtype), ctypes.c_int64(src.stride(0)), _lib.ptr(chunks), chunks.shape[0], int(vec), _lib.ptr_array(dst_ptrs), len(dst_ptrs),
                            _lib.dtype_code(dst_dtype), ctypes.c_int64(dst_pitch), ctypes.c_int64(row_base), src.shape[0], ctypes.c_float(scale), _lib.stream_ptr(src.device))
     _lib.check(code, "trb_grad_push")
+
+
+def grad_push_fp8(src: torch.Tensor, chunks: torch.Tensor, row_dim: int, dst_ptrs: List[int], scale_ptrs: List[int], dst_pitch: int, scale_pitch: int,
+                  row_base: int) -> None:
+    """FP8 variant of ``grad_push`` (native kernel ``trb_grad_push_fp8``): every chunk is a group of ``row_dim`` columns, stored as e4m3
+    payload into ``dst_ptrs`` (uint8 rows of ``dst_pitch`` bytes) and one fp32 scale into ``scale_ptrs`` (rows of ``scale_pitch`` scales)."""
+    assert src.dim() == 2 and src.stride(1) == 1 and chunks.dtype == torch.int32 and chunks.is_contiguous()
+    L = _lib.lib()
+    code = L.trb_grad_push_fp8(_lib.ptr(src), _lib.dtype_code(src.dtype), ctypes.c_int64(src.stride(0)), _lib.ptr(chunks), chunks.shape[0], int(row_dim),
+                               _lib.ptr_array(dst_ptrs), _lib.ptr_array(scale_ptrs), len(dst_ptrs), ctypes.c_int64(dst_pitch), ctypes.c_int64(scale_pitch),
+                               ctypes.c_int64(row_base), src.shape[0], _lib.stream_ptr(src.device))
+    _lib.check(code, "trb_grad_push_fp8")
+
+
+def fp8_wire_decode(payload_ptr: int, pay_pitch: int, scale_ptr: int, scale_pitch: int, row_dim: int, cols: torch.Tensor, rows: int, out: torch.Tensor) -> None:
+    """``out[r, c : c + 16]`` = FP8 payload + scales decoded to ``out.dtype``, for every 16-column chunk start ``c`` in ``cols`` (int32)."""
+    assert out.stride(1) == 1 and cols.dtype == torch.int32
+    L = _lib.lib()
+    code = L.trb_fp8_wire_decode(ctypes.c_void_p(payload_ptr), ctypes.c_int64(pay_pitch), ctypes.c_void_p(scale_ptr), ctypes.c_int64(scale_pitch), int(row_dim),
+                                 _lib.ptr(cols), cols.numel(), ctypes.c_int64(rows), _lib.ptr(out), _lib.dtype_code(out.dtype), ctypes.c_int64(out.stride(0)),
+                                 _lib.stream_ptr(out.device))
+    _lib.check(code, "trb_fp8_wire_decode")

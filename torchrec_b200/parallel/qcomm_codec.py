@@ -3,7 +3,10 @@
 ``CommType`` FP32 / FP16 / BF16 / FP8 / INT8 wire formats for the pooled all-to-all, reduce-scatter and
 sequence all-to-all of the portable transport. FP8 / INT8 are row-wise scaled (one fp32 scale per ``row_dim``
 elements) and therefore not usable for reductions on the wire: reduce-scatter falls back to BF16 (FP16 on CPU).
-The fused NVLink path applies its wire dtype (bf16) inside the kernels and does not need a codec object."""
+
+The fused NVLink plane (``sparse_plane.py``) reads ``fp8_row_dim`` of the codecs: an FP8 row-wise codec makes its kernels carry the
+pooled rows and the gradients of directly written columns as e4m3 groups of that many columns plus one fp32 scale (the arithmetic
+of ``trb_qcomm_encode`` / ``trb_qcomm_decode``, csrc/qcomm_fp8.cuh). Every other codec leaves the plane at its wire dtype."""
 from __future__ import annotations
 
 import logging
@@ -74,6 +77,10 @@ class _CastCodec:
     @property
     def quantized_dtype(self) -> torch.dtype:
         return self._dtype
+
+    @property
+    def fp8_row_dim(self) -> Optional[int]:
+        return None
 
     def calc_quantized_size(self, input_len: int, ctx=None) -> int:
         return input_len
@@ -155,6 +162,11 @@ class _RowwiseCodec:
     def quantized_dtype(self) -> torch.dtype:
         return torch.uint8
 
+    @property
+    def fp8_row_dim(self) -> Optional[int]:
+        """Elements per fp32 scale when this is the FP8 row-wise codec, ``None`` for INT8."""
+        return self._row_dim if self._fp8 else None
+
     def calc_quantized_size(self, input_len: int, ctx=None) -> int:
         return self._rows(input_len) * (self._row_dim + self._tail)
 
@@ -210,6 +222,10 @@ class _Mx4Codec:
     @property
     def quantized_dtype(self) -> torch.dtype:
         return torch.uint8
+
+    @property
+    def fp8_row_dim(self) -> Optional[int]:
+        return None
 
     def calc_quantized_size(self, input_len: int, ctx=None) -> int:
         return (input_len + 31) // 32 * 17

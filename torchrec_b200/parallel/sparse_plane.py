@@ -27,11 +27,18 @@ Slot discipline (what makes the fixed buffers race free; B = barrier of the phas
   out      slot 0 in training (a peer's forward(i+1) is behind its backward barrier of step i, which we only reach after our
                     dense backward(i) consumed out(i)); slots 1/2 alternate for forward-only steps.
   inbox    1 slot   peers push gradients of step i only after the forward barrier of step i, i.e. after our tbe_bwd(i-1).
+
+FP8 wire (``wire_format``): when the engine's quantized-comms codecs ask for FP8 row-wise, the lookup stores directly written pooled
+rows as e4m3 groups of R columns plus one fp32 scale per group into an FP8 region of the out slot, and the gradient push does the
+same into an FP8 inbox; after the barrier one decode launch per direction fills the out slot / inbox in the wire dtype, so
+``out_local`` and ``inbox_local`` keep their meaning. Row-sharded (staged) columns stay at the wire dtype: they are summed at the
+destination, and a row-scaled format cannot be summed on the wire.
 """
 from __future__ import annotations
 
 import ctypes
 import itertools
+import logging
 import os
 from dataclasses import dataclass
 from typing import Any, Dict, List, Optional, Sequence, Tuple
@@ -43,6 +50,10 @@ from ..ops import tbe as T
 from .p2p import SymmetricBuffer, tensor_from_ptr
 
 INT64_MAX = (1 << 63) - 1
+FP8_ROW_DIMS = (32, 64, 128)  # a group of R columns is R / 4 float4 lanes of the lookup kernels, R / 8 lanes of the push: inside one warp
+
+logger = logging.getLogger(__name__)
+_logged_reasons: set = set()
 
 
 def _align(x: int, a: int = 256) -> int:
@@ -124,6 +135,35 @@ class SingleRankGroup:
 
 
 # ---------------------------------------------------------------------------------------------------------------
+def select_wire_format(world: int, direct_cols: Sequence[Tuple[int, int]], push_cols: Sequence[Tuple[int, int, int]],
+                       codecs) -> Tuple[Dict[str, Optional[Tuple[str, int]]], List[str]]:
+    """What each direction of a plane carries: ``{"fwd": ("fp8", R) | None, "bwd": ("fp8", R) | None}`` (``None``: the wire dtype).
+
+    ``direct_cols``: (output column, width) of every directly written unit, the columns the forward may quantize (row-sharded
+    units are summed at the destination and keep the wire dtype); ``push_cols``: (output column, inbox column, width) of every unit
+    the gradient push serves. A direction is FP8 when its codec reports ``fp8_row_dim`` R (FP8 row-wise), R is 32, 64 or 128 and
+    every column offset and width of that direction is a multiple of R; one rank sends nothing over a wire. Also returns the
+    reasons an FP8 direction was refused."""
+    fmt: Dict[str, Optional[Tuple[str, int]]] = {"fwd": None, "bwd": None}
+    why: List[str] = []
+    if world <= 1 or codecs is None:
+        return fmt, why
+    spans = {"fwd": list(direct_cols), "bwd": [(c, w) for c, _i, w in push_cols] + [(i, w) for _c, i, w in push_cols]}
+    for d, codec in (("fwd", getattr(codecs, "forward", None)), ("bwd", getattr(codecs, "backward", None))):
+        R = getattr(codec, "fp8_row_dim", None)
+        if R is None or not spans[d]:
+            continue
+        if R not in FP8_ROW_DIMS:
+            why.append(f"{d}: FP8 row dim {R} is not one of {FP8_ROW_DIMS}")
+            continue
+        bad = [(c, w) for c, w in spans[d] if c % R or w % R]
+        if bad:
+            why.append(f"{d}: the column block at {bad[0][0]} of width {bad[0][1]} is not aligned to the FP8 row dim {R}")
+            continue
+        fmt[d] = ("fp8", R)
+    return fmt, why
+
+
 @dataclass
 class RoutedIds:
     """Handle of a batch whose ids sit in receive slot ``slot`` of ``plane`` (what the input dist of the NVLink plane returns
@@ -245,6 +285,18 @@ class SparsePlane:
         self.staged_width = max(4, (sc + 3) // 4 * 4) if staged_cols else 0
         self.has_staged = bool(staged_cols)
         self.stage_slab_bytes = _align(B_local * self.staged_width * esz) if self.has_staged else 0
+        # ---- wire format (the user's quantized-comms codecs) -----------------------------------------------------------
+        direct = [u for u in units if not eng._table_row_sharded[u.shard.table_idx]]
+        push_cols = [(base_f[u.feature] + u.shard.col_off, local_cols_per_rank[u.shard.rank][i - eng._unit_start[u.shard.rank]], u.shard.cols)
+                     for i, u in enumerate(units)]
+        self.wire_format, why = select_wire_format(W, [(base_f[u.feature] + u.shard.col_off, u.shard.cols) for u in direct], push_cols,
+                                                   getattr(eng, "_codecs", None))
+        for msg in why:
+            if msg not in _logged_reasons:
+                _logged_reasons.add(msg)
+                logger.warning(f"NVLink sparse plane keeps its {self.wire_dtype} wire: {msg}")
+        self.fwd_q = self.wire_format["fwd"][1] if self.wire_format["fwd"] else 0  # FP8 row dim of the forward, 0 = wire dtype
+        self.bwd_q = self.wire_format["bwd"][1] if self.wire_format["bwd"] else 0
         self.id_off = [i * self.id_slot_bytes for i in range(self.N_ID_SLOTS)]
         o = self.N_ID_SLOTS * self.id_slot_bytes
         self.out_off = [o + i * self.slab_bytes for i in range(self.N_OUT_SLOTS)]
@@ -253,6 +305,26 @@ class SparsePlane:
         o += self.inbox_bytes
         self.staging_off = o
         o += self.stage_slab_bytes * W
+        # FP8 regions follow everything else: without an FP8 direction the layout above is all there is
+        if self.fwd_q:  # per out slot: payload [B_local, fq_pitch] uint8 + scales [B_local, fq_spitch] fp32
+            self.fq_pitch, self.fq_spitch = _align(total_cols, 16), (total_cols + self.fwd_q - 1) // self.fwd_q
+            self.fq_off: List[Tuple[int, int]] = []
+            for _ in range(self.N_OUT_SLOTS):
+                pay = _align(B_local * self.fq_pitch)
+                self.fq_off.append((o, o + pay))
+                o += pay + _align(B_local * self.fq_spitch * 4)
+            self.fq_cols = mk32(sorted({base_f[u.feature] + u.shard.col_off + c for u in direct for c in range(0, u.shard.cols, 16)}))
+        if self.bwd_q:  # inbox: payload [W * B_local, bq_pitch] uint8 + scales [W * B_local, bq_spitch] fp32
+            R = self.bwd_q
+            self.bq_pitch, self.bq_spitch = _align(self.inbox_pitch, 16), (self.inbox_pitch + R - 1) // R
+            pay = _align(W * B_local * self.bq_pitch)
+            self.bq_off = (o, o + pay)
+            o += pay + _align(W * B_local * self.bq_spitch * 4)
+            # (destination rank, gradient column, inbox column) of every R-column group
+            self.bq_chunks = torch.tensor([[u.shard.rank, c + k, i + k] for u, (c, i, w) in zip(units, push_cols) for k in range(0, w, R)],
+                                          dtype=torch.int32, device=dev).reshape(-1, 3).contiguous()
+            local_width = sum(u.shard.cols for u in eng._local_units)
+            self.bq_cols = mk32(list(range(0, local_width, 16)))
         self.buf = group.alloc(o)
 
         # staged column bookkeeping for the reduce: contributors + destination column per staged 4-column vector
@@ -445,16 +517,24 @@ class SparsePlane:
         eng = self.eng
         out_ptrs = self.buf.peer_ptrs(self.out_off[out_slot])
         stage_ptrs = [p + self.staging_off + self.rank * self.stage_slab_bytes for p in self.buf.ptrs]
+        fp8 = None
+        if self.fwd_q:  # direct columns go to the FP8 region of the out slot
+            pay, sc = self.fq_off[out_slot]
+            out_ptrs = self.buf.peer_ptrs(pay)
+            fp8 = (self.buf.peer_ptrs(sc), self.fq_spitch, self.fwd_q)
         if local_only:  # measurement aid (bench.py): the same lookup with every destination aliased to local memory = no NVLink traffic
-            out_ptrs = [self.buf.local_ptr + self.out_off[out_slot]] * self.W
+            out_ptrs = [self.buf.local_ptr + (self.fq_off[out_slot][0] if self.fwd_q else self.out_off[out_slot])] * self.W
             stage_ptrs = [self.buf.local_ptr + self.staging_off + self.rank * self.stage_slab_bytes] * self.W
+            if fp8 is not None:
+                fp8 = ([self.buf.local_ptr + self.fq_off[out_slot][1]] * self.W, self.fq_spitch, self.fwd_q)
+        out_pitch = self.fq_pitch if self.fwd_q else self.total_cols
         for g, gm in zip(eng._groups, self.group_meta):
             if gm is None:
                 continue
             u0, _ = g.unit_range
             mean = g.pooling == T.PoolingMode.MEAN
             if gm["direct"] is not None:
-                T.pooled_forward_regions(gm["direct"], g.tbe.weights, reg.window(u0), mean, self.wire_dtype, out_ptrs, self.total_cols, self.B_local, self.device)
+                T.pooled_forward_regions(gm["direct"], g.tbe.weights, reg.window(u0), mean, self.wire_dtype, out_ptrs, out_pitch, self.B_local, self.device, fp8=fp8)
             if gm["staged"] is not None:
                 T.pooled_forward_regions(gm["staged"], g.tbe.weights, reg.window(u0 + gm["n_direct"]), False, self.wire_dtype, stage_ptrs, self.staged_width,
                                          self.B_local, self.device)
@@ -469,6 +549,27 @@ class SparsePlane:
                                          ctypes.c_int64(self.total_cols), ctypes.c_int64(self.stage_slab_bytes // torch.empty(0, dtype=self.wire_dtype).element_size()),
                                          self.W, _lib.stream_ptr(self.device))
         _lib.check(code, "trb_staging_reduce_cols")
+
+    def _decode_out(self, out_slot: int) -> None:
+        """FP8 payload + scales of the direct columns -> the out slot in the wire dtype (after the barrier; disjoint from the staged
+        columns the staging reduce writes)."""
+        if not self.fwd_q:
+            return
+        from . import p2p
+
+        pay, sc = self.fq_off[out_slot]
+        p2p.fp8_wire_decode(self.buf.local_ptr + pay, self.fq_pitch, self.buf.local_ptr + sc, self.fq_spitch, self.fwd_q, self.fq_cols, self.B_local,
+                            self.out_local(out_slot))
+
+    def _decode_inbox(self) -> None:
+        """FP8 gradient inbox -> ``inbox_local()`` in the wire dtype (after the barrier, before the fused backward reads it)."""
+        if not self.bwd_q:
+            return
+        from . import p2p
+
+        pay, sc = self.bq_off
+        p2p.fp8_wire_decode(self.buf.local_ptr + pay, self.bq_pitch, self.buf.local_ptr + sc, self.bq_spitch, self.bwd_q, self.bq_cols, self.W * self.B_local,
+                            self.inbox_local())
 
     def forward(self, ids, training: bool) -> Tuple[torch.Tensor, int]:
         """Lookup + pooled output dist of the batch in ``ids``; returns (local ``[B_local, total_cols]`` output, out slot)."""
@@ -490,6 +591,7 @@ class SparsePlane:
         self._forward_kernels(reg, out_slot)
         self.group.barrier(0)
         self._staging_reduce(out_slot)
+        self._decode_out(out_slot)
 
     # lock-step halves for the loopback driver
     def forward_kernels(self, ids, out_slot: int = 0) -> None:
@@ -498,12 +600,17 @@ class SparsePlane:
 
     def forward_finish(self, out_slot: int = 0) -> torch.Tensor:
         self._staging_reduce(out_slot)
+        self._decode_out(out_slot)
         return self.out_local(out_slot)
 
     # ---- phase 3: gradient dist + fused optimizer ----------------------------------------------------------------------
     def _push_kernels(self, grad: torch.Tensor) -> None:
         from . import p2p
 
+        if self.bwd_q:
+            p2p.grad_push_fp8(grad, self.bq_chunks, self.bwd_q, self.buf.peer_ptrs(self.bq_off[0]), self.buf.peer_ptrs(self.bq_off[1]), self.bq_pitch,
+                              self.bq_spitch, self.rank * self.B_local)
+            return
         p2p.grad_push(grad, self.chunks, self.buf.peer_ptrs(self.inbox_off), self.wire_dtype, self.inbox_pitch, self.rank * self.B_local, 1.0, self.push_vec)
 
     def _backward_kernels(self, reg: T.IdRegions, id_slot: Optional[int], grad_scale: float, phase: int, want_psw: bool = False,
@@ -535,6 +642,7 @@ class SparsePlane:
 
     def _apply_kernels(self, reg: T.IdRegions, id_slot: Optional[int], grad_scale: float, want_psw: bool, grad: Optional[torch.Tensor] = None) -> None:
         prepared = id_slot is not None and self._prepared[id_slot] is not None
+        self._decode_inbox()
         self._backward_kernels(reg, id_slot, grad_scale, phase=2 if prepared else 0, want_psw=want_psw, grad=grad)
 
     def backward(self, ids, grad: torch.Tensor, grad_scale: float, want_psw: bool = False) -> None:

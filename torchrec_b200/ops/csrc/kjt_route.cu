@@ -18,9 +18,11 @@
 //                  raises a device flag that the host reads back asynchronously in the same step.
 //
 // With one destination pointing at local memory the same kernels produce the routed (unit-ordered) KJT for the NCCL / gloo
-// fallback transport, plus the `unbucketize` permutation the sequence (unpooled) path needs.
+// fallback transport, plus the `unbucketize` permutation the sequence (unpooled) path needs. `trb_kjt_route_pos` adds a per-destination
+// payload for the fused sequence inference path: next to every routed id, its position inside its feature's values (where its row goes).
 #include "common.cuh"
 #include <cub/device/device_scan.cuh>
+#include <type_traits>
 
 struct RouteParams {
   const void* in_off;       // [K * B + 1] offsets of the local KJT
@@ -49,6 +51,29 @@ struct RouteParams {
   int64_t capacity;
   int32_t U, B, n_dest, fc;
   int32_t in_off64, val64, out_off64, out_val64;
+};
+
+// Route with a per-destination position payload (trb_kjt_route_pos): next to every routed id its position inside its feature's values,
+// j - in_off[key(u) * B], as int32. A separate type, so the parameter block and the code of the plain route kernels stay as they were.
+struct RoutePosParams : RouteParams {
+  TrbPeerPtrs out_pos;      // per destination: MY region's positions [capacity]
+};
+
+template <class P> constexpr bool kRoutePos = std::is_same_v<P, RoutePosParams>;
+
+// The position store of a writer: nothing for RouteParams.
+template <class P> struct RoutePosOut {
+  __device__ __forceinline__ void init(const P&, int, int) {}
+  __device__ __forceinline__ void st(int64_t, int64_t) {}
+};
+template <> struct RoutePosOut<RoutePosParams> {
+  int32_t* dst;
+  int64_t fs;  // first value of the unit's feature
+  __device__ __forceinline__ void init(const RoutePosParams& p, int u, int d) {
+    dst = reinterpret_cast<int32_t*>(p.out_pos.p[d]);
+    fs = trb_ld_idx(p.in_off, (int64_t) p.u_key[u] * p.B, p.in_off64);
+  }
+  __device__ __forceinline__ void st(int64_t k, int64_t j) { dst[k] = (int32_t) (j - fs); }
 };
 
 __device__ __forceinline__ bool route_full(const RouteParams& p, int u) { return p.u_row_lo[u] == 0 && p.u_row_hi[u] == INT64_MAX; }
@@ -95,7 +120,8 @@ __global__ void __launch_bounds__(256) kjt_route_len_kernel(const RouteParams p)
 // ---- C: write offsets + ids into the destination regions -------------------------------------------------------------------
 // One thread per (unit, sample): consecutive threads handle consecutive samples of one unit, i.e. consecutive source ids and
 // consecutive destination positions for short bags (one-hot features: fully coalesced 8 B loads / peer stores).
-__global__ void __launch_bounds__(256) kjt_route_write_kernel(const RouteParams p) {
+template <class P>
+__device__ __forceinline__ void route_write(const P p) {
   const int64_t t = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
   const int64_t n = (int64_t) p.U * p.B;
   if (t >= n) return;
@@ -118,6 +144,8 @@ __global__ void __launch_bounds__(256) kjt_route_write_kernel(const RouteParams 
   const int64_t lo = p.u_row_lo[u], hi = p.u_row_hi[u];
   const bool full = route_full(p, u);  // whole-table units forward EVERY id (invalid ones are zeroed by the lookup kernel)
   float* const wdst = reinterpret_cast<float*>(p.out_wgt.p[d]);
+  RoutePosOut<P> po;
+  po.init(p, u, d);
   int64_t k = o;
   for (int64_t j = s; j < e; ++j) {
     const int64_t id = trb_ld_idx(p.in_val, j, p.val64);
@@ -127,15 +155,20 @@ __global__ void __launch_bounds__(256) kjt_route_write_kernel(const RouteParams 
       trb_st_idx(p.out_val.p[d], k, p.out_val64, local);
       if (p.in_wgt != nullptr) wdst[k] = p.in_wgt[j];
       if (p.pos_out != nullptr) p.pos_out[k] = j - s;
+      po.st(k, j);
     }
     if (p.unbucketize != nullptr) p.unbucketize[j * p.fc + p.u_cslice[u]] = k + base;
     ++k;
   }
 }
 
+__global__ void __launch_bounds__(256) kjt_route_write_kernel(const RouteParams p) { route_write(p); }
+__global__ void __launch_bounds__(256) kjt_route_write_pos_kernel(const RoutePosParams p) { route_write(p); }
+
 // Long bags: one warp per (unit, sample), lanes stride over the bag; row-range filtering keeps the source order through a
 // ballot prefix (ids of one bag stay in input order, which the sequence path relies on).
-__global__ void __launch_bounds__(256) kjt_route_write_warp_kernel(const RouteParams p) {
+template <class P>
+__device__ __forceinline__ void route_write_warp(const P p) {
   const int lane = threadIdx.x & 31;
   const int64_t t = ((int64_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int64_t n = (int64_t) p.U * p.B;
@@ -161,6 +194,8 @@ __global__ void __launch_bounds__(256) kjt_route_write_warp_kernel(const RoutePa
   const int64_t lo = p.u_row_lo[u], hi = p.u_row_hi[u];
   const bool full = route_full(p, u);
   float* const wdst = reinterpret_cast<float*>(p.out_wgt.p[d]);
+  RoutePosOut<P> po;
+  po.init(p, u, d);
   int64_t k0 = o;
   for (int64_t j0 = s; j0 < e; j0 += 32) {
     const int64_t j = j0 + lane;
@@ -178,12 +213,16 @@ __global__ void __launch_bounds__(256) kjt_route_write_warp_kernel(const RoutePa
         trb_st_idx(p.out_val.p[d], k, p.out_val64, local);
         if (p.in_wgt != nullptr) wdst[k] = p.in_wgt[j];
         if (p.pos_out != nullptr) p.pos_out[k] = j - s;
+        po.st(k, j);
       }
       if (p.unbucketize != nullptr) p.unbucketize[j * p.fc + p.u_cslice[u]] = k + base;
     }
     k0 += __popc(m);
   }
 }
+
+__global__ void __launch_bounds__(256) kjt_route_write_warp_kernel(const RouteParams p) { route_write_warp(p); }
+__global__ void __launch_bounds__(256) kjt_route_write_warp_pos_kernel(const RoutePosParams p) { route_write_warp(p); }
 
 static inline size_t route_align(size_t x) { return (x + 255) & ~(size_t) 255; }
 
@@ -198,19 +237,19 @@ TRB_API int64_t trb_kjt_route_workspace_bytes(int U, int B) {
   return (int64_t) (2 * route_align(n * 4) + route_align(route_scan_tmp_bytes(n)) + 256);
 }
 
-// Returns 0 on success. `avg_len_hint` (ids per bag, host estimate) picks the thread-per-bag or warp-per-bag writer.
-TRB_API int trb_kjt_route_ex(const void* in_off, int in_off64, const void* in_val, int val64, const float* in_wgt, int B, const int32_t* u_key,
-                             const int64_t* u_row_lo, const int64_t* u_row_hi, const int32_t* u_dest, const int32_t* u_slot,
-                             const int32_t* u_cslice, const int32_t* dest_ustart, int U, int n_dest, void* const* out_off_ptrs, int out_off64,
-                             void* const* out_val_ptrs, int out_val64, void* const* out_wgt_ptrs, int64_t capacity, int64_t* unbucketize, int fc,
-                             int64_t* pos_out, const int64_t* u_wrap, const int32_t* u_wrap_rem, int wrap_mod, const int32_t* u_edge, int32_t* lengths_out,
-                             int32_t* overflow, void* workspace, int64_t workspace_bytes, int avg_len_hint, cudaStream_t stream) {
+// Fills the fields of RouteParams and launches the three passes with the writer of P.
+template <class P>
+static int route_run(P& p, const void* in_off, int in_off64, const void* in_val, int val64, const float* in_wgt, int B, const int32_t* u_key,
+                     const int64_t* u_row_lo, const int64_t* u_row_hi, const int32_t* u_dest, const int32_t* u_slot,
+                     const int32_t* u_cslice, const int32_t* dest_ustart, int U, int n_dest, void* const* out_off_ptrs, int out_off64,
+                     void* const* out_val_ptrs, int out_val64, void* const* out_wgt_ptrs, int64_t capacity, int64_t* unbucketize, int fc,
+                     int64_t* pos_out, const int64_t* u_wrap, const int32_t* u_wrap_rem, int wrap_mod, const int32_t* u_edge, int32_t* lengths_out,
+                     int32_t* overflow, void* workspace, int64_t workspace_bytes, int avg_len_hint, cudaStream_t stream) {
   if (n_dest < 1 || n_dest > TRB_MAX_PEERS) return -1;
   if (U == 0 || B == 0) return 0;
   const int64_t n = (int64_t) U * B;
   if (n + 1 >= ((int64_t) 1 << 31)) return -6;
   if (workspace_bytes < trb_kjt_route_workspace_bytes(U, B)) return -7;
-  RouteParams p;
   p.in_off = in_off; p.in_val = in_val; p.in_wgt = in_wgt;
   p.u_key = u_key; p.u_row_lo = u_row_lo; p.u_row_hi = u_row_hi; p.u_dest = u_dest; p.u_slot = u_slot; p.u_cslice = u_cslice;
   p.dest_ustart = dest_ustart;
@@ -229,17 +268,51 @@ TRB_API int trb_kjt_route_ex(const void* in_off, int in_off64, const void* in_va
   p.U = U; p.B = B; p.n_dest = n_dest; p.fc = fc > 0 ? fc : 1;
   p.in_off64 = in_off64; p.val64 = val64; p.out_off64 = out_off64; p.out_val64 = out_val64;
   const int threads = 256;
-  kjt_route_len_kernel<<<(unsigned) ((n + 1 + threads - 1) / threads), threads, 0, stream>>>(p);
+  kjt_route_len_kernel<<<(unsigned) ((n + 1 + threads - 1) / threads), threads, 0, stream>>>(static_cast<const RouteParams&>(p));
   TRB_CHECK_LAUNCH();
   TRB_CUDA(cub::DeviceScan::ExclusiveSum(scan_tmp, scan_tmp_bytes, (const int32_t*) p.len, p.scan, (int) (n + 1), stream));
   g_trb_launches += 1;
   if (avg_len_hint > 8) {
-    kjt_route_write_warp_kernel<<<(unsigned) ((n * 32 + threads - 1) / threads), threads, 0, stream>>>(p);
+    const unsigned blocks = (unsigned) ((n * 32 + threads - 1) / threads);
+    if constexpr (kRoutePos<P>) kjt_route_write_warp_pos_kernel<<<blocks, threads, 0, stream>>>(p);
+    else kjt_route_write_warp_kernel<<<blocks, threads, 0, stream>>>(p);
   } else {
-    kjt_route_write_kernel<<<(unsigned) ((n + threads - 1) / threads), threads, 0, stream>>>(p);
+    const unsigned blocks = (unsigned) ((n + threads - 1) / threads);
+    if constexpr (kRoutePos<P>) kjt_route_write_pos_kernel<<<blocks, threads, 0, stream>>>(p);
+    else kjt_route_write_kernel<<<blocks, threads, 0, stream>>>(p);
   }
   TRB_CHECK_LAUNCH();
   return 0;
+}
+
+// Returns 0 on success. `avg_len_hint` (ids per bag, host estimate) picks the thread-per-bag or warp-per-bag writer.
+TRB_API int trb_kjt_route_ex(const void* in_off, int in_off64, const void* in_val, int val64, const float* in_wgt, int B, const int32_t* u_key,
+                             const int64_t* u_row_lo, const int64_t* u_row_hi, const int32_t* u_dest, const int32_t* u_slot,
+                             const int32_t* u_cslice, const int32_t* dest_ustart, int U, int n_dest, void* const* out_off_ptrs, int out_off64,
+                             void* const* out_val_ptrs, int out_val64, void* const* out_wgt_ptrs, int64_t capacity, int64_t* unbucketize, int fc,
+                             int64_t* pos_out, const int64_t* u_wrap, const int32_t* u_wrap_rem, int wrap_mod, const int32_t* u_edge, int32_t* lengths_out,
+                             int32_t* overflow, void* workspace, int64_t workspace_bytes, int avg_len_hint, cudaStream_t stream) {
+  RouteParams p;
+  return route_run(p, in_off, in_off64, in_val, val64, in_wgt, B, u_key, u_row_lo, u_row_hi, u_dest, u_slot, u_cslice, dest_ustart, U, n_dest,
+                   out_off_ptrs, out_off64, out_val_ptrs, out_val64, out_wgt_ptrs, capacity, unbucketize, fc, pos_out, u_wrap, u_wrap_rem, wrap_mod,
+                   u_edge, lengths_out, overflow, workspace, workspace_bytes, avg_len_hint, stream);
+}
+
+// The route of the sequence inference path: ids (no weights) plus, per destination, the int32 position of every routed id inside its
+// feature's values (`out_pos_ptrs`, [capacity] each). `n_in` = number of input ids; more than INT32_MAX of them cannot be addressed by
+// the int32 positions and returns -8. `u_edge` as in trb_kjt_route_ex (may be null).
+TRB_API int trb_kjt_route_pos(const void* in_off, int in_off64, const void* in_val, int val64, int64_t n_in, int B, const int32_t* u_key,
+                              const int64_t* u_row_lo, const int64_t* u_row_hi, const int32_t* u_dest, const int32_t* u_slot, const int32_t* dest_ustart,
+                              const int32_t* u_edge, int U, int n_dest, void* const* out_off_ptrs, int out_off64, void* const* out_val_ptrs, int out_val64,
+                              void* const* out_pos_ptrs, int64_t capacity, int32_t* overflow, void* workspace, int64_t workspace_bytes, int avg_len_hint,
+                              cudaStream_t stream) {
+  if (n_in > INT32_MAX) return -8;
+  if (n_dest < 1 || n_dest > TRB_MAX_PEERS) return -1;
+  RoutePosParams p;
+  for (int i = 0; i < TRB_MAX_PEERS; ++i) p.out_pos.p[i] = i < n_dest ? out_pos_ptrs[i] : nullptr;
+  return route_run(p, in_off, in_off64, in_val, val64, nullptr, B, u_key, u_row_lo, u_row_hi, u_dest, u_slot, nullptr, dest_ustart, U, n_dest,
+                   out_off_ptrs, out_off64, out_val_ptrs, out_val64, nullptr, capacity, nullptr, 1, nullptr, nullptr, nullptr, 1, u_edge, nullptr,
+                   overflow, workspace, workspace_bytes, avg_len_hint, stream);
 }
 
 TRB_API int trb_kjt_route(const void* in_off, int in_off64, const void* in_val, int val64, const float* in_wgt, int B, const int32_t* u_key,

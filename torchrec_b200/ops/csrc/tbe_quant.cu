@@ -506,6 +506,131 @@ __global__ void __launch_bounds__(256) qtbe_seq_kernel(const QP<PLACED> p, int64
   }
 }
 
+// ---- sequence scatter (fused sharded sequence inference, trb_qtbe_seq_scatter) ---------------------------------------------------------
+// The ids of a launch were routed by trb_kjt_route_pos: `offsets` ([F * B + 1], region-absolute, the first entry need not be 0) slice the
+// routed ids into units f, and pos[k] is the position of routed id k inside its feature's values. The dequantized row of id k of unit f is
+// stored at out + feat_obase[f] + pos[k] * feat_ostride[f] + feat_col[f] (out: the flat sequence output on the first device, so from any
+// other device these are peer stores). Ids outside the unit's rows store zeros.
+template <bool PLACED>
+struct QTbeScatter : QP<PLACED> {  // derived, so the parameter block of the qtbe_* instances above stays as it was
+  const int64_t* feat_obase;   // element offset of the unit's feature block in `out`
+  const int32_t* feat_ostride; // the feature's full width D_f
+  const int32_t* pos;          // [routed ids] position of the id inside its feature's values
+};
+
+// Routed id of thread group t (region-absolute index) and its unit; false past the last routed id (the grid covers a host-side bound).
+template <bool PLACED>
+__device__ __forceinline__ bool qscatter_id(const QTbeScatter<PLACED>& p, int64_t t, int64_t& i, int& f) {
+  i = trb_ld_idx(p.offsets, 0, p.off64) + t;
+  if (i >= trb_ld_idx(p.offsets, (int64_t) p.F * p.B, p.off64)) return false;
+  int lo = 0, hi = p.F - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (trb_ld_idx(p.offsets, (int64_t) mid * p.B, p.off64) <= i) lo = mid; else hi = mid - 1;
+  }
+  f = lo;
+  return true;
+}
+
+// Row of a routed id (clamped to row 0 when invalid) with the cache bookkeeping of qtbe_seq_kernel, kept by lane `keeper` only.
+template <bool PLACED>
+__device__ __forceinline__ const uint8_t* qscatter_row(const QTbeScatter<PLACED>& p, int f, int64_t idx, bool ok, bool keeper) {
+  if constexpr (PLACED) {
+    const QPlace pl = qplace(p, f);
+    int32_t slot;
+    const uint8_t* row = qrow(pl, ok ? idx : 0, p.feat_row_bytes[f], slot);
+    if (keeper && ok && pl.ct >= 0) {
+      qcache_note(p.ctabs[pl.ct], idx, slot);
+      QCount cnt;
+      cnt.add(p.ctabs, pl.ct, slot);
+      cnt.flush(p.ctabs);
+    }
+    return row;
+  } else {
+    return p.weights + p.feat_woff[f] + (ok ? idx : 0) * (int64_t) p.feat_row_bytes[f];
+  }
+}
+
+template <typename O, bool PLACED>
+__device__ __forceinline__ O* qscatter_dst(const QTbeScatter<PLACED>& p, int f, int64_t i) {
+  return reinterpret_cast<O*>(p.out) + p.feat_obase[f] + (int64_t) p.pos[i] * p.feat_ostride[f] + p.feat_col[f];
+}
+
+// any row formats: one warp per routed id, 4 elements per lane (as qtbe_seq_kernel)
+template <typename O, bool PLACED>
+__global__ void __launch_bounds__(256) qtbe_seq_scatter_kernel(const QTbeScatter<PLACED> p, int64_t bound) {
+  const int lane = threadIdx.x & 31;
+  const int64_t t = ((int64_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  int64_t i;
+  int f;
+  if (t >= bound || !qscatter_id(p, t, i, f)) return;
+  const int D = p.feat_dim[f];
+  const int fmt = p.feat_fmt[f];
+  const int64_t idx = trb_ld_idx(p.indices, i, p.idx64);
+  const bool ok = idx >= 0 && idx < p.feat_rows[f];
+  const uint8_t* row = qscatter_row(p, f, idx, ok, lane == 0);
+  O* dst = qscatter_dst<O>(p, f, i);
+  for (int vi = lane; vi < (D >> 2); vi += 32) {
+    const float4 v = ok ? dequant4(row, fmt, D, vi * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
+    Vec4<O>::st(dst + vi * 4, v);
+  }
+}
+
+// one of INT8 / FP8 block-scaled / FP16 / BF16 / INT4 for every table of the launch, rows of whole 16-byte vectors: 8 lanes per routed
+// id, one 16 B vector (EPV elements) per lane and step (the loads and the dequantization of qtbe_fwd_vec_kernel)
+template <typename O, int FMT, bool PLACED>
+__global__ void __launch_bounds__(256) qtbe_seq_scatter_vec_kernel(const QTbeScatter<PLACED> p, int64_t bound) {
+  constexpr int LPR = 8;
+  constexpr int EPV = QVec<FMT>::EPV;
+  const int lig = threadIdx.x & (LPR - 1);
+  const int64_t t = ((int64_t) blockIdx.x * blockDim.x + threadIdx.x) / LPR;
+  int64_t i;
+  int f;
+  if (t >= bound || !qscatter_id(p, t, i, f)) return;
+  const int D = p.feat_dim[f];
+  const int64_t idx = trb_ld_idx(p.indices, i, p.idx64);
+  const bool ok = idx >= 0 && idx < p.feat_rows[f];
+  const uint8_t* row = qscatter_row(p, f, idx, ok, lig == 0);
+  O* dst = qscatter_dst<O>(p, f, i);
+  for (int e = lig * EPV; e < D; e += LPR * EPV) {
+    float v[EPV];
+    if (ok) {
+      dequant_vec<FMT>(*reinterpret_cast<const uint4*>(row + (e / EPV) * 16), load_scale_vec<FMT>(row, D, e), v);
+    } else {
+#pragma unroll
+      for (int k = 0; k < EPV; ++k) v[k] = 0.f;
+    }
+    store_vec<O, EPV>(dst + e, v);
+  }
+}
+
+template <typename O, bool PLACED>
+static int launch_q_scatter(const QTbeScatter<PLACED>& p, int64_t bound, int uniform_fmt, cudaStream_t stream) {
+  const int threads = 256;
+  const unsigned vec_blocks = (unsigned) ((bound * 8 + threads - 1) / threads);
+  switch (uniform_fmt) {  // (the caller guarantees rows made of whole 16-byte vectors: quant_tbe.py _uniform_fmt)
+    case FMT_FP8_BLOCK: qtbe_seq_scatter_vec_kernel<O, FMT_FP8_BLOCK, PLACED><<<vec_blocks, threads, 0, stream>>>(p, bound); break;
+    case FMT_INT8: qtbe_seq_scatter_vec_kernel<O, FMT_INT8, PLACED><<<vec_blocks, threads, 0, stream>>>(p, bound); break;
+    case FMT_FP16: qtbe_seq_scatter_vec_kernel<O, FMT_FP16, PLACED><<<vec_blocks, threads, 0, stream>>>(p, bound); break;
+    case FMT_BF16: qtbe_seq_scatter_vec_kernel<O, FMT_BF16, PLACED><<<vec_blocks, threads, 0, stream>>>(p, bound); break;
+    case FMT_INT4: qtbe_seq_scatter_vec_kernel<O, FMT_INT4, PLACED><<<vec_blocks, threads, 0, stream>>>(p, bound); break;
+    default: qtbe_seq_scatter_kernel<O, PLACED><<<(unsigned) ((bound * 32 + threads - 1) / threads), threads, 0, stream>>>(p, bound);
+  }
+  TRB_CHECK_LAUNCH();
+  return 0;
+}
+
+template <bool PLACED>
+static int launch_q_scatter_out(const QTbeScatter<PLACED>& p, int out_dtype, int64_t bound, int uniform_fmt, cudaStream_t stream) {
+  if (bound <= 0 || p.F == 0 || p.B == 0) return 0;
+  switch (out_dtype) {
+    case TRB_F32: return launch_q_scatter<float, PLACED>(p, bound, uniform_fmt, stream);
+    case TRB_F16: return launch_q_scatter<__half, PLACED>(p, bound, uniform_fmt, stream);
+    case TRB_BF16: return launch_q_scatter<__nv_bfloat16, PLACED>(p, bound, uniform_fmt, stream);
+  }
+  return -3;
+}
+
 template <typename O, bool PLACED>
 static int launch_q(const QP<PLACED>& p, int max_dim, int64_t total, int uniform_fmt, cudaStream_t stream) {
   const int threads = 256;
@@ -582,6 +707,32 @@ TRB_API int trb_qtbe_fwd_placed(const int64_t* feat_base, const int32_t* feat_ct
   p.feat_row_bytes = feat_row_bytes; p.indices = indices; p.offsets = offsets; p.psw = psw; p.out = out; p.out_stride = out_stride;
   p.B = B; p.F = F; p.idx64 = idx64; p.off64 = off64; p.mean = mean; p.pooled = pooled;
   return launch_q_out<true>(p, out_dtype, max_dim, total, uniform_fmt, stream);
+}
+
+// Sequence scatter lookup over F units of B bags (see QTbeScatter). HBM tables: `weights` + `feat_woff`, `feat_base` null; placed tables
+// (any of them in host memory or behind an HBM row cache): `feat_base`, `feat_ctab`, `ctabs`, `no_slot` as in trb_qtbe_fwd_placed.
+// `bound` >= the number of routed ids of the launch (sizes the grid; the kernels stop at offsets[F * B]). `uniform_fmt` as in trb_qtbe_fwd_ex.
+TRB_API int trb_qtbe_seq_scatter(const void* weights, const int64_t* feat_woff, const int64_t* feat_base, const int32_t* feat_ctab, const void* ctabs,
+                                 const int32_t* no_slot, const int64_t* feat_rows, const int32_t* feat_dim, const int32_t* feat_col, const int32_t* feat_fmt,
+                                 const int32_t* feat_row_bytes, const int64_t* feat_obase, const int32_t* feat_ostride, const void* indices, int idx64,
+                                 const void* offsets, int off64, const int32_t* pos, void* out, int out_dtype, int B, int F, int64_t bound, int uniform_fmt,
+                                 cudaStream_t stream) {
+  auto fill = [&](auto& p) {
+    p.feat_rows = feat_rows; p.feat_dim = feat_dim; p.feat_col = feat_col; p.feat_fmt = feat_fmt; p.feat_row_bytes = feat_row_bytes;
+    p.indices = indices; p.offsets = offsets; p.psw = nullptr; p.out = out; p.out_stride = 0;
+    p.B = B; p.F = F; p.idx64 = idx64; p.off64 = off64; p.mean = 0; p.pooled = 0;
+    p.feat_obase = feat_obase; p.feat_ostride = feat_ostride; p.pos = pos;
+  };
+  if (feat_base != nullptr) {
+    QTbeScatter<true> p{};
+    fill(p);
+    p.feat_base = feat_base; p.feat_ctab = feat_ctab; p.ctabs = reinterpret_cast<const QCacheTab*>(ctabs); p.no_slot = no_slot;
+    return launch_q_scatter_out<true>(p, out_dtype, bound, uniform_fmt, stream);
+  }
+  QTbeScatter<false> p{};
+  fill(p);
+  p.weights = reinterpret_cast<const uint8_t*>(weights); p.feat_woff = feat_woff;
+  return launch_q_scatter_out<false>(p, out_dtype, bound, uniform_fmt, stream);
 }
 
 // ---- admission: claimed misses -> HBM slots ---------------------------------------------------------------------------------------------

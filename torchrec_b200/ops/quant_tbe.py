@@ -345,6 +345,29 @@ class QuantTableBatchedEmbeddingBags(nn.Module):
         _lib.check(code, "trb_qtbe_fwd_ex")
         return out
 
+    def forward_scatter(self, indices: torch.Tensor, offsets: torch.Tensor, pos: torch.Tensor, B: int, out: torch.Tensor, feat_obase: torch.Tensor,
+                        feat_ostride: torch.Tensor, feat_col: torch.Tensor, bound: int) -> None:
+        """Sequence lookup over routed ids (``trb_qtbe_seq_scatter``). ``offsets`` (int32 / int64, ``F * B + 1`` entries, the first need
+        not be 0) slice ``indices`` and ``pos`` (int32, the position of each id inside its feature's values). The row of routed id k of
+        feature f is stored at ``out + feat_obase[f] + pos[k] * feat_ostride[f] + feat_col[f]`` (int64 / int32 / int32, one entry per
+        feature; ``out`` may live on another device with peer access enabled). ``bound`` >= the number of routed ids. Placed tables wait
+        for the last admission first and admit the rows this lookup missed afterwards."""
+        L = _lib.lib()
+        F = len(self.feature_table_map)
+        if self._placed:
+            self._wait_admission()
+            where = [None, None, _lib.ptr(self.feat_base), _lib.ptr(self.feat_ctab), _lib.ptr(self.cache_tabs), _lib.ptr(self.no_slot)]
+        else:
+            where = [_lib.ptr(self.weights), _lib.ptr(self.feat_woff), None, None, None, None]
+        code = L.trb_qtbe_seq_scatter(*where, _lib.ptr(self.feat_rows), _lib.ptr(self.feat_dim), _lib.ptr(feat_col), _lib.ptr(self.feat_fmt),
+                                      _lib.ptr(self.feat_rb), _lib.ptr(feat_obase), _lib.ptr(feat_ostride), _lib.ptr(indices),
+                                      int(indices.dtype == torch.int64), _lib.ptr(offsets), int(offsets.dtype == torch.int64), _lib.ptr(pos), _lib.ptr(out),
+                                      _lib.dtype_code(self.output_dtype), B, F, ctypes.c_int64(bound), int(self._uniform_fmt),
+                                      _lib.stream_ptr(self.weights.device))
+        _lib.check(code, "trb_qtbe_seq_scatter")
+        if self._placed and self._cached:
+            self._admit()
+
     def _ref_forward(self, indices, offsets, psw, B: int, pooled: bool) -> torch.Tensor:
         offsets = offsets.long()
         indices = indices.long()

@@ -54,6 +54,25 @@ def _lib():
     return _LIB
 
 
+def batch_views(buf: torch.Tensor, d: "_BatchDesc", id_list_keys: Sequence[str], id_score_list_keys: Sequence[str]):
+    """``(dense [B, num_float] | None, id_list KJT | None, id_score_list KJT | None)`` as views of one batch slab ``buf`` (host or device)."""
+    B = d.batch_size
+
+    def view(off, n, dtype, esz):
+        return buf[off : off + n * esz].view(dtype)
+
+    dense = view(d.dense_off, B * d.num_float, torch.float32, 4).view(B, d.num_float) if d.num_float else None
+    kjt = wkjt = None
+    if d.id_list_features:
+        kjt = KeyedJaggedTensor(keys=id_list_keys, values=view(d.idl_values_off, d.idl_num_values, torch.int64, 8),
+                                lengths=view(d.idl_lengths_off, B * d.id_list_features, torch.int32, 4), stride=B)
+    if d.id_score_features:
+        wkjt = KeyedJaggedTensor(keys=id_score_list_keys, values=view(d.ids_values_off, d.ids_num_values, torch.int64, 8),
+                                 lengths=view(d.ids_lengths_off, B * d.id_score_features, torch.int32, 4),
+                                 weights=view(d.ids_weights_off, d.ids_num_values, torch.float32, 4), stride=B)
+    return dense, kjt, wkjt
+
+
 @dataclass
 class ServerConfig:
     max_batch_size: int = 2048
@@ -68,14 +87,27 @@ class ServerConfig:
 
 class InferenceServer:
     """``predict_fn(dense [B, num_float] | None, id_list KJT | None, id_score_list KJT | None) -> Tensor [B] or [B, P]``,
-    one callable per device."""
+    one callable per device. A captured ``inference.graphed.GraphedPredictor`` may stand in for a callable: its batches replay a CUDA
+    graph from the predictor's static device slab."""
 
     def __init__(self, predict_fns: Sequence[Callable], devices: Sequence[torch.device], id_list_keys: Sequence[str] = (), id_score_list_keys: Sequence[str] = (),
                  config: Optional[ServerConfig] = None) -> None:
+        from .graphed import GraphedPredictor
+
         assert len(predict_fns) == len(devices) and len(devices) >= 1
         self.cfg = config or ServerConfig()
         self.devices = [torch.device(d) for d in devices]
         self.predict_fns = list(predict_fns)
+        self._graphed = [isinstance(fn, GraphedPredictor) for fn in self.predict_fns]
+        for fn, dev, g in zip(self.predict_fns, self.devices, self._graphed):
+            if g and (dev.type != "cuda" or not fn.captured or fn.device != dev or fn.buffer_bytes < self.cfg.buffer_bytes
+                      or fn.max_batch_size < self.cfg.max_batch_size or fn.id_list_keys != list(id_list_keys)
+                      or fn.id_score_list_keys != list(id_score_list_keys)):
+                raise ValueError(f"a GraphedPredictor serves the CUDA device it was captured on, after capture(), with the server's keys, a slab "
+                                 f"of at least buffer_bytes={self.cfg.buffer_bytes} and max_batch_size >= {self.cfg.max_batch_size} (got device "
+                                 f"{dev}, captured={fn.captured}, {fn.device}, {fn.buffer_bytes} bytes, max_batch_size={fn.max_batch_size}, "
+                                 f"keys {fn.id_list_keys} / {fn.id_score_list_keys})")
+        self._out_host: List[Optional[torch.Tensor]] = [None] * len(self.devices)
         self.id_list_keys, self.id_score_list_keys = list(id_list_keys), list(id_score_list_keys)
         L = _lib()
         self._h = L.trb_srv_create(self.cfg.max_batch_size, int(self.cfg.batching_interval_ms * 1000), len(self.devices), self.cfg.max_outstanding_per_gpu,
@@ -135,26 +167,28 @@ class InferenceServer:
     def _tensors(self, slab: torch.Tensor, d: _BatchDesc, dev: torch.device):
         host = slab[: d.total_bytes]
         buf = host.to(dev, non_blocking=True) if dev.type == "cuda" else host  # ONE copy per batch
-        B = d.batch_size
+        return batch_views(buf, d, self.id_list_keys, self.id_score_list_keys)
 
-        def view(off, n, dtype, esz):
-            return buf[off : off + n * esz].view(dtype)
-
-        dense = view(d.dense_off, B * d.num_float, torch.float32, 4).view(B, d.num_float) if d.num_float else None
-        kjt = wkjt = None
-        if d.id_list_features:
-            kjt = KeyedJaggedTensor(keys=self.id_list_keys, values=view(d.idl_values_off, d.idl_num_values, torch.int64, 8),
-                                    lengths=view(d.idl_lengths_off, B * d.id_list_features, torch.int32, 4), stride=B)
-        if d.id_score_features:
-            wkjt = KeyedJaggedTensor(keys=self.id_score_list_keys, values=view(d.ids_values_off, d.ids_num_values, torch.int64, 8),
-                                     lengths=view(d.ids_lengths_off, B * d.id_score_features, torch.int32, 4),
-                                     weights=view(d.ids_weights_off, d.ids_num_values, torch.float32, 4), stride=B)
-        return dense, kjt, wkjt
+    def _run_graphed(self, gpu: int, slab: torch.Tensor, d: _BatchDesc, stream) -> torch.Tensor:
+        """A ``GraphedPredictor``: the slab goes into its static device slab (the one H2D copy), the result back through a pinned buffer."""
+        gp = self.predict_fns[gpu]
+        n = d.total_bytes
+        gp.slab[:n].copy_(slab[:n], non_blocking=True)
+        out = gp.run(gp.slab, d).reshape(d.batch_size, -1)
+        if self._out_host[gpu] is None or self._out_host[gpu].numel() < out.numel():
+            self._out_host[gpu] = torch.empty(max(out.numel(), self.cfg.max_batch_size * self.cfg.outputs_per_sample), dtype=torch.float32, pin_memory=True)
+        res = self._out_host[gpu][: out.numel()].view(out.shape)
+        res.copy_(out, non_blocking=True)
+        stream.synchronize()
+        if gp.ingest_failed():
+            raise RuntimeError("serve_ingest rejected the batch")
+        return res
 
     def _executor(self, gpu: int) -> None:
         L = _lib()
         dev = self.devices[gpu]
         stream = torch.cuda.Stream(dev) if dev.type == "cuda" else None
+        graphed = self._graphed[gpu]
         d = _BatchDesc()
         while not self._stop:
             rc = L.trb_srv_pop_batch(self._h, gpu, 50_000, ctypes.byref(d))
@@ -164,7 +198,10 @@ class InferenceServer:
                 continue
             try:
                 with torch.inference_mode():
-                    if stream is not None:
+                    if graphed:
+                        with torch.cuda.stream(stream):
+                            out = self._run_graphed(gpu, self._slabs[d.buffer_index], d, stream)
+                    elif stream is not None:
                         with torch.cuda.stream(stream):
                             out = self.predict_fns[gpu](*self._tensors(self._slabs[d.buffer_index], d, dev))
                             out = out.float().reshape(d.batch_size, -1).cpu()

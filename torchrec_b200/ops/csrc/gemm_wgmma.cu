@@ -3,22 +3,28 @@
 // and a fused epilogue (bias, ReLU / sigmoid, ReLU-gradient mask, ReLU bit mask, bias-gradient column sums,
 // bf16 / fp32 store or split-K fp32 reduction).
 //
-// Two kernels share the mainloop and the epilogue:
+// Three kernels share the TMA producer, the wgmma k-block and the epilogue:
 //
-// N > 64: gemm_bf16_wgmma_persistent_kernel, 128 x BN tiles (BN = 256; 128 for N <= 128 and for split-K at N <= 256), one CTA per SM walking a static
-// tile list (tile i, i + gridDim.x, ...; consecutive tiles share an A row-block, so the CTAs running at once read the same A rows):
-//   warps 0..3   consumer warpgroup 0   rows [0, 64) of the tile:   4 x wgmma m64nBNk16 per 64-wide k-block
-//   warps 4..7   consumer warpgroup 1   rows [64, 128) of the tile
-//   warps 8..11  producer warpgroup     one thread issues cp.async.bulk.tensor.2d -> smem ring (kStages x (A 128x64, B BNx64))
-// setmaxnreg moves registers from the producer warpgroup (40) to the consumers (232): 128 fp32 accumulators per thread at BN = 256.
-// The producer runs ahead into the next tile's k-blocks while the consumers run the epilogue. A bf16 output without split-K leaves
-// through shared memory: each consumer warpgroup writes its 64 x BN block into a SWIZZLE_128B staging buffer and one thread issues
-// TMA stores (64 x 64 boxes, clipped at M / N by the tensor map), then the warpgroup returns to its MMAs; the staging buffer is
-// reused once the previous tile's stores have read it. fp32 / split-K outputs (and outputs a tensor map cannot describe) are stored
-// from the fragment layout.
+// N > 128, bf16 output without split-K (but not a plain MN-major-B product, see gemm_dispatch): gemm_bf16_wgmma_pingpong_kernel,
+// one CTA per SM walking a static list of 128 x 128 tiles (tile i, i + gridDim.x, ...; consecutive tiles share an A row-block, so
+// the CTAs running at once read the same A rows):
+//   warps 0..3   consumer warpgroup 0   the 1st, 3rd, ... tile of the list: 2 x 4 wgmma m64n128k16 per 64-wide k-block
+//   warps 4..7   consumer warpgroup 1   the 2nd, 4th, ... tile
+//   warps 8..11  producer warpgroup     one thread issues cp.async.bulk.tensor.2d -> smem ring (4 x (A 128x64, B 128x64)), in list order
+// setmaxnreg moves registers from the producer warpgroup (40) to the consumers (232): 128 fp32 accumulators per thread. The two
+// mainloops alternate (ordered mbarrier pair), so one warpgroup's epilogue runs while the other's MMAs keep the tensor cores busy;
+// with the cooperative schedule below, every epilogue left them idle, a share of the tile that grows as K shrinks (a 128 x 256 tile
+// has 8 k-blocks at K = 512, 2 at K = 128). The output leaves through shared memory: the warpgroup writes its tile into a
+// SWIZZLE_128B staging buffer and one thread issues TMA stores (64 x 64 boxes, clipped at M / N by the tensor map); the buffer is
+// reused once the warpgroup's previous stores have read it. Outputs a tensor map cannot describe are stored from the fragment layout.
+//
+// Other N > 64 (fp32 / split-K outputs such as the weight gradients, whose K is the batch; N <= 128; plain MN-major-B products):
+// gemm_bf16_wgmma_persistent_kernel, cooperative: the same producer and CTA walk over 128 x BN tiles (BN = 256; 128 for N <= 128
+// and for split-K at N <= 256), consumer warpgroup w computes rows [64 w, 64 w + 64) of each tile with 4 x wgmma m64nBNk16 per
+// k-block, and both run the tile's epilogue; a bf16 output leaves through a 64 x BN staging buffer per warpgroup and TMA stores.
 //
 // N <= 64: gemm_bf16_wgmma_kernel, one 128 x 64 tile per CTA and two CTAs per SM (one CTA's epilogue overlaps the other's MMAs);
-// warps 0..7 are the consumers as above, warp 8 the TMA producer.
+// warps 0..7 are the consumers as in the cooperative kernel, warp 8 the TMA producer.
 //
 // A consumer keeps one wgmma group in flight and releases the previous k-block's slot when it retires.
 //
@@ -61,7 +67,7 @@ struct GemmParams {
   // 32-row slab of the bf16 output go to colsum_ws[row0 / 32][n] ([ceil(M / 32), N], deterministic; reduced by
   // trb_colsum_partials). nullptr: not wanted.
   float* colsum_ws;
-  int tma_out;                  // 1: bf16 output through shared memory and TMA stores (persistent kernel, split_k == 1)
+  int tma_out;                  // 1: bf16 output through shared memory and TMA stores (persistent kernels, split_k == 1)
 };
 
 __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
@@ -84,7 +90,10 @@ struct SmemLayout {
 // ACT / BIAS are compile-time so the unrolled loop carries no runtime branches on them.
 // STAGED: the bf16 values go to `stage` (BN / 64 SWIZZLE_128B boxes of 64 rows x 64 columns) for a TMA store instead of global memory,
 // and the bias of columns [n0, n0 + BN) is read from `bias_s` (shared memory; a register-resident bias spills at BN = 256).
-template <int BN, int ACT, bool BIAS, bool STAGED>
+// WORD_ONCE: with mask_bits, load the mask word of each row and 32 columns once and keep it in a register for the 4 fragment column
+// groups it covers (instead of once per group of 8 columns). Off in the cooperative kernel: there the hoisted loads change the
+// register allocation of the whole kernel, and its plain and fp32 variants (weight gradients, plain dgrads) measured slower.
+template <int BN, int ACT, bool BIAS, bool STAGED, bool WORD_ONCE>
 __device__ __forceinline__ void epilogue_impl(const GemmParams& p, float (&acc)[BN / 2], int row0, int n0, int wq, int lane, float* colsum_s,
                                               uint8_t* stage, const float* bias_s) {
   const int q = lane & 3;
@@ -93,10 +102,17 @@ __device__ __forceinline__ void epilogue_impl(const GemmParams& p, float (&acc)[
   const bool want_colsum = p.colsum_ws != nullptr;
   const bool use_bits = (ACT == ACT_RELU_GRAD) && p.mask_bits != nullptr;
   uint32_t obits[2] = {0u, 0u};
+  uint32_t mword[2] = {0u, 0u};  // WORD_ONCE: the mask words of columns [n0 + 8 (j & ~3), + 32)
 #pragma unroll
   for (int j = 0; j < BN / 8; ++j) {
     const int col = n0 + 8 * j + 2 * q;
     const bool col_ok = col < p.N;  // N % 8 == 0: col + 1 < N as well
+    if (WORD_ONCE && use_bits && (j & 3) == 0) {
+      // n0 is a multiple of 32: the 4 j of this word share column word (col >> 5); a word past N is never read (col_ok below)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        mword[h] = row_ok[h] && col_ok ? __ldg(p.mask_bits + (int64_t) rows[h] * p.ld_bits + (col >> 5)) : 0u;
+    }
     float2 b2 = make_float2(0.f, 0.f);
     if constexpr (BIAS) {
       if constexpr (STAGED) {
@@ -125,7 +141,7 @@ __device__ __forceinline__ void epilogue_impl(const GemmParams& p, float (&acc)[
       } else if constexpr (ACT == ACT_RELU_GRAD) {
         if (ok) {
           if (use_bits) {
-            const uint32_t w = __ldg(p.mask_bits + (int64_t) rows[h] * p.ld_bits + (col >> 5)) >> (col & 31);
+            const uint32_t w = (WORD_ONCE ? mword[h] : __ldg(p.mask_bits + (int64_t) rows[h] * p.ld_bits + (col >> 5))) >> (col & 31);
             v0 = (w & 1u) ? v0 : 0.f;
             v1 = (w & 2u) ? v1 : 0.f;
           } else {
@@ -205,10 +221,10 @@ __device__ __forceinline__ void epilogue_impl(const GemmParams& p, float (&acc)[
   }
 }
 
-template <int BN, bool STAGED>
+template <int BN, bool STAGED, bool WORD_ONCE>
 __device__ __forceinline__ void epilogue(const GemmParams& p, float (&acc)[BN / 2], int row0, int n0, int wq, int lane, float* colsum_s,
                                          uint8_t* stage = nullptr, const float* bias_s = nullptr) {
-#define TRB_EPI(A, B) epilogue_impl<BN, A, B, STAGED>(p, acc, row0, n0, wq, lane, colsum_s, stage, bias_s)
+#define TRB_EPI(A, B) epilogue_impl<BN, A, B, STAGED, WORD_ONCE>(p, acc, row0, n0, wq, lane, colsum_s, stage, bias_s)
   const bool bias = p.bias != nullptr;
   switch (p.act) {
     case ACT_RELU: if (bias) TRB_EPI(ACT_RELU, true); else TRB_EPI(ACT_RELU, false); break;
@@ -321,7 +337,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
   wgmma_wait<0>();
   wgmma_fence_regs(acc);
   // (no arrival for the last slot: nothing is loaded after this tile's last k-block)
-  epilogue<BN, false>(p, acc, m_blk * BLOCK_M + 64 * wg, n_blk * BN, wq, lane, reinterpret_cast<float*>(smem + L::kColsumOffset) + wg * 2 * BN);
+  epilogue<BN, false, true>(p, acc, m_blk * BLOCK_M + 64 * wg, n_blk * BN, wq, lane, reinterpret_cast<float*>(smem + L::kColsumOffset) + wg * 2 * BN);
 }
 
 constexpr int kPersistentThreads = kConsumerThreads + 128;
@@ -341,8 +357,61 @@ struct PersistentLayout {
   static_assert(kTotal + 1024 <= 227 * 1024, "shared memory of one CTA per SM");
 };
 
+// Ping-pong kernel: 128 x 128 tiles, one per consumer warpgroup.
+struct PingPongLayout {
+  static constexpr int BN = 128;
+  static constexpr int kStages = 4;
+  static constexpr int kABytes = BLOCK_M * BLOCK_K * 2;
+  static constexpr int kBBytes = BN * BLOCK_K * 2;
+  static constexpr int kStageBytes = kABytes + kBBytes;
+  static constexpr int kOutOffset = kStages * kStageBytes;             // [2 warpgroups][2 row halves][64 rows x BN] bf16 staging
+  static constexpr int kOutBytes = BLOCK_M * BN * 2;                   // per warpgroup
+  static constexpr int kColsumOffset = kOutOffset + 2 * kOutBytes;     // [2 warpgroups][2 row halves][2 slabs][BN] fp32
+  static constexpr int kBiasOffset = kColsumOffset + 8 * BN * 4;      // [2 warpgroups][BN] fp32 bias of the tile's columns
+  static constexpr int kBarOffset = kBiasOffset + 2 * BN * 4;         // full[kStages], empty[kStages], order[2]
+  static constexpr int kTotal = kBarOffset + (2 * kStages + 2) * 8;
+  static_assert(kTotal + 1024 <= 227 * 1024, "shared memory of one CTA per SM");
+};
+
 __device__ __forceinline__ void warpgroup_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
 
+// TMA producer of the persistent kernels (one thread): the k-blocks of the CTA's work items (item i, i + gridDim.x, ...), in list
+// order, into the ring of kStages slots of A 128 x 64 + B BN x 64.
+template <int BN, int kStages, bool A_MN, bool B_MN>
+__device__ __forceinline__ void produce(const CUtensorMap* tmap_a, const CUtensorMap* tmap_b, uint8_t* smem, uint64_t* full_bar,
+                                        uint64_t* empty_bar, int items, int mn_tiles, int n_tiles, int k_blocks_total, int kb_per_split) {
+  constexpr int kABytes = BLOCK_M * BLOCK_K * 2, kStageBytes = kABytes + BN * BLOCK_K * 2;
+  asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tmap_a)) : "memory");
+  asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tmap_b)) : "memory");
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int item = blockIdx.x; item < items; item += gridDim.x) {
+    const int mn = item % mn_tiles, ks = item / mn_tiles;
+    const int m_blk = mn / n_tiles, n_blk = mn % n_tiles;
+    const int kb0 = ks * kb_per_split, kb1 = min(k_blocks_total, kb0 + kb_per_split);
+    for (int kb = kb0; kb < kb1; ++kb) {
+      mbar_wait(&empty_bar[stage], phase ^ 1);
+      uint8_t* sa = smem + stage * kStageBytes;
+      uint8_t* sb = sa + kABytes;
+      mbar_arrive_expect_tx(&full_bar[stage], kStageBytes);
+      if constexpr (A_MN) {
+#pragma unroll
+        for (int h = 0; h < BLOCK_M / 64; ++h) tma_load_2d(tmap_a, &full_bar[stage], sa + h * 8192, m_blk * BLOCK_M + 64 * h, kb * BLOCK_K);
+      } else {
+        tma_load_2d(tmap_a, &full_bar[stage], sa, kb * BLOCK_K, m_blk * BLOCK_M);
+      }
+      if constexpr (B_MN) {
+#pragma unroll
+        for (int h = 0; h < BN / 64; ++h) tma_load_2d(tmap_b, &full_bar[stage], sb + h * 8192, n_blk * BN + 64 * h, kb * BLOCK_K);
+      } else {
+        tma_load_2d(tmap_b, &full_bar[stage], sb, kb * BLOCK_K, n_blk * BN);
+      }
+      if (++stage == kStages) { stage = 0; phase ^= 1; }
+    }
+  }
+}
+
+// Cooperative schedule: both consumer warpgroups work on one 128 x BN tile, rows [0, 64) and [64, 128), and both run its epilogue.
 // TMA_OUT: bf16 output through the staging buffer and TMA stores (p.tma_out); otherwise stores from the fragment layout.
 template <int BN, bool A_MN, bool B_MN, bool TMA_OUT>
 __global__ void __launch_bounds__(kPersistentThreads, 1)
@@ -377,36 +446,8 @@ gemm_bf16_wgmma_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, co
   if (warp_idx >= kConsumerThreads / 32) {
     // ================= TMA producer warpgroup =================
     setmaxnreg_dec<40>();
-    if (warp_idx == kConsumerThreads / 32 && lane == 0) {
-      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmap_a)) : "memory");
-      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmap_b)) : "memory");
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int item = blockIdx.x; item < items; item += gridDim.x) {
-        const int mn = item % mn_tiles, ks = item / mn_tiles;
-        const int m_blk = mn / n_tiles, n_blk = mn % n_tiles;
-        const int kb0 = ks * kb_per_split, kb1 = min(k_blocks_total, kb0 + kb_per_split);
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sa = smem + stage * L::kStageBytes;
-          uint8_t* sb = sa + L::kABytes;
-          mbar_arrive_expect_tx(&full_bar[stage], L::kStageBytes);
-          if constexpr (A_MN) {
-#pragma unroll
-            for (int h = 0; h < BLOCK_M / 64; ++h) tma_load_2d(&tmap_a, &full_bar[stage], sa + h * 8192, m_blk * BLOCK_M + 64 * h, kb * BLOCK_K);
-          } else {
-            tma_load_2d(&tmap_a, &full_bar[stage], sa, kb * BLOCK_K, m_blk * BLOCK_M);
-          }
-          if constexpr (B_MN) {
-#pragma unroll
-            for (int h = 0; h < BN / 64; ++h) tma_load_2d(&tmap_b, &full_bar[stage], sb + h * 8192, n_blk * BN + 64 * h, kb * BLOCK_K);
-          } else {
-            tma_load_2d(&tmap_b, &full_bar[stage], sb, kb * BLOCK_K, n_blk * BN);
-          }
-          if (++stage == kStages) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
+    if (warp_idx == kConsumerThreads / 32 && lane == 0)
+      produce<BN, kStages, A_MN, B_MN>(&tmap_a, &tmap_b, smem, full_bar, empty_bar, items, mn_tiles, n_tiles, k_blocks_total, kb_per_split);
     return;
   }
 
@@ -453,7 +494,7 @@ gemm_bf16_wgmma_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, co
         for (int c = threadIdx.x & 127; c < BN; c += 128) bias_s[c] = n0 + c < p.N ? p.bias[n0 + c] : 0.f;
         warpgroup_sync(wg);
       }
-      epilogue<BN, true>(p, acc, row0, n0, wq, lane, colsum_s, out_stage, bias_s);
+      epilogue<BN, true, false>(p, acc, row0, n0, wq, lane, colsum_s, out_stage, bias_s);
       fence_proxy_async();
       warpgroup_sync(wg);
       if (leader && row0 < p.M) {
@@ -464,7 +505,154 @@ gemm_bf16_wgmma_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, co
       }
     } else {
       warpgroup_sync(wg);  // every warp is past the previous epilogue: colsum_s is free
-      epilogue<BN, false>(p, acc, row0, n0, wq, lane, colsum_s);
+      epilogue<BN, false, false>(p, acc, row0, n0, wq, lane, colsum_s);
+    }
+  }
+  if constexpr (TMA_OUT) {
+    if (leader) tma_store_wait_all();
+  }
+}
+
+// One 64-wide k-block of a 128 x 128 tile by one warpgroup: per k16 step two wgmma m64n128k16, rows [0, 64) and [64, 128).
+template <bool A_MN, bool B_MN>
+__device__ __forceinline__ void mma_kblock_m128(float (&acc)[2][64], uint32_t a_addr, uint32_t b_addr) {
+#pragma unroll
+  for (int k = 0; k < BLOCK_K / WGMMA_K; ++k) {
+    const uint64_t bd = B_MN ? make_smem_desc(b_addr + k * 2048, 8192, 1024) : make_kmajor_desc(b_addr + k * 32);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      // A rows [64 h, 64 h + 64): K-major = 64 rows x 128 B further; MN-major = the second 64-column atom
+      const uint32_t ah = a_addr + (uint32_t) h * 8192u;
+      const uint64_t ad = A_MN ? make_smem_desc(ah + k * 2048, 8192, 1024) : make_kmajor_desc(ah + k * 32);
+      wgmma_m64n128k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc[h], ad, bd);
+    }
+  }
+}
+
+// Ping-pong schedule (bf16 outputs without split-K, routed by gemm_dispatch): each consumer warpgroup owns whole 128 x 128 tiles and the two take
+// alternate tiles of the CTA's list (tile i, i + gridDim.x, ...: warpgroup 0 the 1st, 3rd, ..., warpgroup 1 the 2nd, 4th, ...).
+// An ordered pair of mbarriers makes their mainloops alternate: a warpgroup starts a tile's MMAs once the other one has issued
+// the last MMAs of the previous tile, so one warpgroup's epilogue runs while the other multiplies. The producer fills one ring in
+// list order; each slot is read by one warpgroup.
+// TMA_OUT: bf16 output through the staging buffer and TMA stores (p.tma_out); otherwise stores from the fragment layout.
+template <bool A_MN, bool B_MN, bool TMA_OUT>
+__global__ void __launch_bounds__(kPersistentThreads, 1)
+gemm_bf16_wgmma_pingpong_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                                const __grid_constant__ CUtensorMap tmap_out, const GemmParams p) {
+  using L = PingPongLayout;
+  constexpr int BN = L::BN, kStages = L::kStages;
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t) 1023);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::kBarOffset);
+  uint64_t* empty_bar = full_bar + kStages;
+  uint64_t* order_bar = empty_bar + kStages;  // order_bar[w]: warpgroup w may start its next mainloop
+
+  const int warp_idx = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < kStages; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], 1);  // one arrival by the warpgroup that read the slot
+    }
+    mbar_init(&order_bar[0], 1);
+    mbar_init(&order_bar[1], 1);
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  const int n_tiles = (p.N + BN - 1) / BN;
+  const int tiles = ((p.M + BLOCK_M - 1) / BLOCK_M) * n_tiles;
+  const int k_blocks = (p.K + BLOCK_K - 1) / BLOCK_K;
+
+  if (warp_idx >= kConsumerThreads / 32) {
+    // ================= TMA producer warpgroup =================
+    setmaxnreg_dec<40>();
+    if (warp_idx == kConsumerThreads / 32 && lane == 0)
+      produce<BN, kStages, A_MN, B_MN>(&tmap_a, &tmap_b, smem, full_bar, empty_bar, tiles, tiles, n_tiles, k_blocks, k_blocks);
+    return;
+  }
+
+  // ================= consumers =================
+  setmaxnreg_inc<232>();
+  const int wg = warp_idx >> 2;
+  const int wq = warp_idx & 3;
+  const bool leader = (threadIdx.x & 127) == 0;
+  uint8_t* out_stage = smem + L::kOutOffset + wg * L::kOutBytes;
+  float* colsum_s = reinterpret_cast<float*>(smem + L::kColsumOffset) + wg * 4 * BN;
+  float* bias_s = reinterpret_cast<float*>(smem + L::kBiasOffset) + wg * BN;
+  // Parity of the next order_bar[wg] phase to wait for. Warpgroup 0 waits for parity 1 first, which a fresh barrier reports as
+  // complete: it starts at once. Each wait is at most one phase behind the other warpgroup's arrivals (it arrives once per tile
+  // and then waits for this warpgroup's arrival), so a parity wait cannot pass early.
+  uint32_t order_phase = wg == 0 ? 1u : 0u;
+  // ring position (k-blocks loaded before) of this warpgroup's next k-block; every tile has k_blocks of them
+  int pos = wg * k_blocks;
+  float acc[2][BN / 2];
+  for (int tile = blockIdx.x + wg * gridDim.x; tile < tiles; tile += 2 * gridDim.x) {
+    const int m_blk = tile / n_tiles, n_blk = tile % n_tiles;
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) {
+      acc[0][i] = 0.f;
+      acc[1][i] = 0.f;
+    }
+    // The other warpgroup has issued every MMA of the previous tile, so it has also seen every k-block before this tile's arrive:
+    // the full_bar slots this tile waits for are at most one phase ahead of what has completed.
+    mbar_wait(&order_bar[wg], order_phase);
+    order_phase ^= 1u;
+    int prev_stage = pos % kStages;
+    for (int kb = 0; kb < k_blocks; ++kb, ++pos) {
+      const int stage = pos % kStages;
+      mbar_wait(&full_bar[stage], (uint32_t) (pos / kStages) & 1u);
+      const uint32_t a_addr = smem_u32(smem + stage * L::kStageBytes);
+      const uint32_t b_addr = a_addr + L::kABytes;
+      wgmma_fence();
+      mma_kblock_m128<A_MN, B_MN>(acc, a_addr, b_addr);
+      wgmma_commit();
+      wgmma_wait<1>();  // the previous k-block's wgmmas retired: its smem slot is free
+      wgmma_fence_regs(acc[0]);
+      wgmma_fence_regs(acc[1]);
+      if (kb > 0 && leader) mbar_arrive(&empty_bar[prev_stage]);
+      prev_stage = stage;
+    }
+    if (leader) mbar_arrive(&order_bar[wg ^ 1]);  // this tile's last MMAs are issued: the other warpgroup's mainloop may start
+    pos += k_blocks;                              // (the other warpgroup's tile)
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc[0]);
+    wgmma_fence_regs(acc[1]);
+    if (leader) mbar_arrive(&empty_bar[prev_stage]);
+    const int row0 = m_blk * BLOCK_M, n0 = n_blk * BN;
+    // the epilogue runs once per 64-row half, each with its own column-sum scratch (no barrier between the two)
+    if constexpr (TMA_OUT) {
+      if (leader) tma_store_wait_read();  // this warpgroup's previous stores have read the staging buffer
+      warpgroup_sync(wg);                 // ... and every warp is past the previous epilogue (colsum_s / bias_s are free as well)
+      if (p.bias != nullptr) {
+        for (int c = threadIdx.x & 127; c < BN; c += 128) bias_s[c] = n0 + c < p.N ? p.bias[n0 + c] : 0.f;
+        warpgroup_sync(wg);
+      }
+      epilogue<BN, true, true>(p, acc[0], row0, n0, wq, lane, colsum_s, out_stage, bias_s);
+      epilogue<BN, true, true>(p, acc[1], row0 + 64, n0, wq, lane, colsum_s + 2 * BN, out_stage + L::kOutBytes / 2, bias_s);
+      fence_proxy_async();
+      warpgroup_sync(wg);
+      if (leader) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+#pragma unroll
+          for (int b = 0; b < BN / 64; ++b)
+            if (row0 + 64 * h < p.M && n0 + 64 * b < p.N)
+              tma_store_2d(&tmap_out, out_stage + h * (L::kOutBytes / 2) + b * 8192, n0 + 64 * b, row0 + 64 * h);
+        }
+        tma_store_commit();
+      }
+    } else {
+      warpgroup_sync(wg);  // every warp is past the previous epilogue: colsum_s is free
+      // (a rolled loop over the halves, the second moved into acc[0] first: two inlined copies of this epilogue spill)
+#pragma unroll 1
+      for (int h = 0; h < 2; ++h) {
+        if (h == 1) {
+#pragma unroll
+          for (int i = 0; i < BN / 2; ++i) acc[0][i] = acc[1][i];
+        }
+        epilogue<BN, false, true>(p, acc[0], row0 + 64 * h, n0, wq, lane, colsum_s + h * 2 * BN);
+      }
     }
   }
   if constexpr (TMA_OUT) {
@@ -519,6 +707,26 @@ int launch_gemm_persistent(const CUtensorMap& ta, const CUtensorMap& tb, const C
   return 0;
 }
 
+template <bool A_MN, bool B_MN>
+int launch_gemm_pingpong(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to, const GemmParams& p, cudaStream_t stream) {
+  constexpr int smem_bytes = PingPongLayout::kTotal + 1024;
+  static bool configured = false;
+  if (!configured) {
+    TRB_CUDA(cudaFuncSetAttribute(gemm_bf16_wgmma_pingpong_kernel<A_MN, B_MN, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
+    TRB_CUDA(cudaFuncSetAttribute(gemm_bf16_wgmma_pingpong_kernel<A_MN, B_MN, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
+    configured = true;
+  }
+  const int64_t tiles = (int64_t) ((p.M + BLOCK_M - 1) / BLOCK_M) * ((p.N + PingPongLayout::BN - 1) / PingPongLayout::BN);
+  if (tiles > 0x7fffffff) return -12;
+  const int grid = (int) (tiles < trb_num_sms() ? tiles : trb_num_sms());
+  if (p.tma_out)
+    gemm_bf16_wgmma_pingpong_kernel<A_MN, B_MN, true><<<grid, kPersistentThreads, smem_bytes, stream>>>(ta, tb, to, p);
+  else
+    gemm_bf16_wgmma_pingpong_kernel<A_MN, B_MN, false><<<grid, kPersistentThreads, smem_bytes, stream>>>(ta, tb, to, p);
+  TRB_CHECK_LAUNCH();
+  return 0;
+}
+
 template <int BN, bool A_MN, bool B_MN>
 int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t stream) {
   constexpr int smem_bytes = SmemLayout<BN>::kTotal + 1024;
@@ -551,23 +759,32 @@ static int gemm_dispatch(const void* A, int64_t lda, const void* B, int64_t ldb,
     if (rc) return rc;
     return launch_gemm<64, A_MN, B_MN>(ta, tb, p, stream);
   }
-  // split-K items of narrow outputs stay 128 wide: the split plans (gemm.py _wgrad_plan) fill the grid with 128 x 128 items, and at
-  // N <= 256 one 128 x 256 item per (m, n) block would leave half the SMs idle
-  const int bn = (p.N <= 128 || (p.split_k > 1 && p.N <= 256)) ? 128 : 256;
-  rc = B_MN ? make_tmap(&tb, B, p.K, p.N, ldb, 64, 64) : make_tmap(&tb, B, p.N, p.K, ldb, bn);
-  if (rc) return rc;
   // bf16 output without split-K: TMA stores of 64 x 64 boxes (needs a 16 B aligned base and row pitch)
   CUtensorMap to;
   memset(&to, 0, sizeof(to));
   p.tma_out = !p.out_f32 && p.split_k == 1 && reinterpret_cast<uintptr_t>(p.out) % 16 == 0 && p.ldo % 8 == 0 &&
               make_tmap(&to, p.out, p.M, p.N, p.ldo, 64, 64) == 0;
+  // Ping-pong for bf16 outputs without split-K, except where the cooperative kernel measured faster (H100, DESIGN.md): N <= 128
+  // (one 128 x 128 tile per row-block, split over both warpgroups) and a plain MN-major-B product (a dgrad without a ReLU mask),
+  // whose bare conversion epilogue gains less from the overlap than 128 x 256 tiles save in operand traffic.
+  const bool plain = p.act == ACT_NONE && p.bias == nullptr && p.colsum_ws == nullptr;
+  if (!p.out_f32 && p.split_k == 1 && p.N > 128 && !(B_MN && plain)) {
+    rc = B_MN ? make_tmap(&tb, B, p.K, p.N, ldb, 64, 64) : make_tmap(&tb, B, p.N, p.K, ldb, PingPongLayout::BN);
+    if (rc) return rc;
+    return launch_gemm_pingpong<A_MN, B_MN>(ta, tb, to, p, stream);
+  }
+  // Cooperative. Split-K items of narrow outputs stay 128 wide: the split plans (gemm.py _wgrad_plan) fill the grid with 128 x 128
+  // items, and at N <= 256 one 128 x 256 item per (m, n) block would leave half the SMs idle
+  const int bn = (p.N <= 128 || (p.split_k > 1 && p.N <= 256)) ? 128 : 256;
+  rc = B_MN ? make_tmap(&tb, B, p.K, p.N, ldb, 64, 64) : make_tmap(&tb, B, p.N, p.K, ldb, bn);
+  if (rc) return rc;
   if (bn == 128) return launch_gemm_persistent<128, A_MN, B_MN>(ta, tb, to, p, stream);
   return launch_gemm_persistent<256, A_MN, B_MN>(ta, tb, to, p, stream);
 }
 
 // mask_bits / relu_bits_out: int32 [M, ld_bits] bit matrices (bit n % 32 of word n / 32), see GemmParams.
 // colsum_ws: fp32 [ceil(M / 32), N] or nullptr, see GemmParams (bf16 output without split-K only: -14 otherwise).
-// tile_n: tile-width hint of the caller's split-K plan; the tile shape depends on N only (128 x 64, 128 x 128 or 128 x 256).
+// tile_n: tile-width hint of the caller's split-K plan; the tile shape depends on N, the output type and split-K only (128 x 64, 128 x 128 or 128 x 256).
 TRB_API int trb_gemm_bf16(const void* A, int64_t lda, int a_mn, const void* B, int64_t ldb, int b_mn, void* out, int64_t ldo, int out_f32, int M,
                           int N, int K, const float* bias, int act, const void* mask, int64_t ld_mask, float alpha, int split_k, int tile_n,
                           const void* mask_bits, void* relu_bits_out, int64_t ld_bits, float* colsum_ws, cudaStream_t stream) {

@@ -34,7 +34,10 @@ def gemm_bf16(a: torch.Tensor, b: torch.Tensor, a_mn: bool = False, b_mn: bool =
               out: Optional[torch.Tensor] = None, split_k: int = 1, tile_n: int = 0, mask_bits: Optional[torch.Tensor] = None,
               relu_bits_out: Optional[torch.Tensor] = None, colsum_ws: Optional[torch.Tensor] = None) -> torch.Tensor:
     """``act(alpha * op(a) @ op(b)^T + bias)`` on the wgmma kernels: 128 x 64 tiles for N <= 64 (two CTAs per SM), otherwise a
-    persistent kernel (one CTA per SM) on 128 x 128 tiles for N <= 128 and 128 x 256 tiles above (128 x 128 for split-K up to N = 256).
+    persistent kernel (one CTA per SM): bf16 outputs without split-K at N > 128 on 128 x 128 tiles, one per consumer warpgroup
+    (ping-pong: one warpgroup's epilogue runs while the other multiplies), unless the product is plain (no bias, activation or column
+    sums) with an MN-major b; otherwise both warpgroups on one tile, 128 x 128 for N <= 128 and 128 x 256 above (128 x 128 for
+    split-K up to N = 256).
     ``tile_n``: the tile width the caller sized ``split_k`` for (a hint; the kernel's tile depends on N and split-K only). ``relu_bits_out`` (int32
     ``[M, ceil(N / 32)]``, with ``ACT_RELU``): receives one bit per output (> 0); ``mask_bits`` (same layout, with ``ACT_RELU_GRAD``): used instead of re-reading ``mask``.
 

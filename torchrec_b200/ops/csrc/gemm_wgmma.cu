@@ -5,9 +5,10 @@
 //
 // Three kernels share the TMA producer, the wgmma k-block and the epilogue:
 //
-// N > 128, bf16 output without split-K (but not a plain MN-major-B product, see gemm_dispatch): gemm_bf16_wgmma_pingpong_kernel,
-// one CTA per SM walking a static list of 128 x 128 tiles (tile i, i + gridDim.x, ...; consecutive tiles share an A row-block, so
-// the CTAs running at once read the same A rows):
+// N > 128, bf16 output without split-K (but not a plain MN-major-B product, see gemm_dispatch), and N > 64 split-K fp32 outputs a
+// tensor map can describe (the weight gradients): gemm_bf16_wgmma_pingpong_kernel, one CTA per SM walking a static list of 128 x 128
+// items (item i, i + gridDim.x, ...; an item is a tile and, with split-K, one K-slice of it; consecutive items share an A row-block,
+// so the CTAs running at once read the same A rows):
 //   warps 0..3   consumer warpgroup 0   the 1st, 3rd, ... tile of the list: 2 x 4 wgmma m64n128k16 per 64-wide k-block
 //   warps 4..7   consumer warpgroup 1   the 2nd, 4th, ... tile
 //   warps 8..11  producer warpgroup     one thread issues cp.async.bulk.tensor.2d -> smem ring (4 x (A 128x64, B 128x64)), in list order
@@ -16,9 +17,11 @@
 // with the cooperative schedule below, every epilogue left them idle, a share of the tile that grows as K shrinks (a 128 x 256 tile
 // has 8 k-blocks at K = 512, 2 at K = 128). The output leaves through shared memory: the warpgroup writes its tile into a
 // SWIZZLE_128B staging buffer and one thread issues TMA stores (64 x 64 boxes, clipped at M / N by the tensor map); the buffer is
-// reused once the warpgroup's previous stores have read it. Outputs a tensor map cannot describe are stored from the fragment layout.
+// reused once the warpgroup's previous stores have read it. A split-K partial tile leaves the same way, as fp32 in two 64-row halves,
+// through TMA reduce-adds into the pre-zeroed output. Outputs a tensor map cannot describe are stored from the fragment layout.
 //
-// Other N > 64 (fp32 / split-K outputs such as the weight gradients, whose K is the batch; N <= 128; plain MN-major-B products):
+// Other N > 64 (N <= 128 bf16; plain MN-major-B products; fp32 outputs without split-K, and split-K outputs whose base or row pitch
+// is not 16 B aligned, reduced with fp32 atomics):
 // gemm_bf16_wgmma_persistent_kernel, cooperative: the same producer and CTA walk over 128 x BN tiles (BN = 256; 128 for N <= 128
 // and for split-K at N <= 256), consumer warpgroup w computes rows [64 w, 64 w + 64) of each tile with 4 x wgmma m64nBNk16 per
 // k-block, and both run the tile's epilogue; a bf16 output leaves through a 64 x BN staging buffer per warpgroup and TMA stores.
@@ -529,18 +532,32 @@ __device__ __forceinline__ void mma_kblock_m128(float (&acc)[2][64], uint32_t a_
   }
 }
 
-// Ping-pong schedule (bf16 outputs without split-K, routed by gemm_dispatch): each consumer warpgroup owns whole 128 x 128 tiles and the two take
-// alternate tiles of the CTA's list (tile i, i + gridDim.x, ...: warpgroup 0 the 1st, 3rd, ..., warpgroup 1 the 2nd, 4th, ...).
-// An ordered pair of mbarriers makes their mainloops alternate: a warpgroup starts a tile's MMAs once the other one has issued
-// the last MMAs of the previous tile, so one warpgroup's epilogue runs while the other multiplies. The producer fills one ring in
+// Output of the ping-pong kernel
+enum PingPongOut : int {
+  PP_DIRECT = 0,   // bf16, stored from the fragment layout (outputs a tensor map cannot describe)
+  PP_TMA = 1,      // bf16 through the staging buffer and TMA stores (p.tma_out)
+  PP_ADD_F32 = 2,  // split-K fp32 (p.split_k > 1, out pre-zeroed): TMA reduce-add of each K-slice's partial tile
+};
+
+// fp32 value pair (row r, columns c, c + 1; c even) of a [64 rows x 32 columns] SWIZZLE_128B box (128 B rows, 16 B chunks XOR r % 8)
+__device__ __forceinline__ uint32_t sw128_offset_f32(int r, int c) {
+  return (uint32_t) (r * 128 + ((((c >> 2) ^ (r & 7)) & 7) << 4) + ((c & 3) << 2));
+}
+
+// Ping-pong schedule (bf16 outputs without split-K, and split-K fp32 outputs; routed by gemm_dispatch): each consumer warpgroup owns
+// whole 128 x 128 items (a tile and, with split-K, one K-slice of it: item = tile + tiles * slice) and the two take alternate items of
+// the CTA's list (item i, i + gridDim.x, ...: warpgroup 0 the 1st, 3rd, ..., warpgroup 1 the 2nd, 4th, ...).
+// An ordered pair of mbarriers makes their mainloops alternate: a warpgroup starts an item's MMAs once the other one has issued
+// the last MMAs of the previous item, so one warpgroup's epilogue runs while the other multiplies. The producer fills one ring in
 // list order; each slot is read by one warpgroup.
-// TMA_OUT: bf16 output through the staging buffer and TMA stores (p.tma_out); otherwise stores from the fragment layout.
-template <bool A_MN, bool B_MN, bool TMA_OUT>
+template <bool A_MN, bool B_MN, int OUT>
 __global__ void __launch_bounds__(kPersistentThreads, 1)
 gemm_bf16_wgmma_pingpong_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                                 const __grid_constant__ CUtensorMap tmap_out, const GemmParams p) {
   using L = PingPongLayout;
   constexpr int BN = L::BN, kStages = L::kStages;
+  constexpr bool TMA_OUT = OUT == PP_TMA;
+  constexpr bool SPLIT = OUT == PP_ADD_F32;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t) 1023);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::kBarOffset);
@@ -563,12 +580,24 @@ gemm_bf16_wgmma_pingpong_kernel(const __grid_constant__ CUtensorMap tmap_a, cons
   const int n_tiles = (p.N + BN - 1) / BN;
   const int tiles = ((p.M + BLOCK_M - 1) / BLOCK_M) * n_tiles;
   const int k_blocks = (p.K + BLOCK_K - 1) / BLOCK_K;
+  // split-K: slice s covers k-blocks [s * kb_per_split, min(k_blocks, (s + 1) * kb_per_split)); trb_gemm_bf16 leaves no slice empty
+  const int splits = SPLIT ? p.split_k : 1;
+  const int kb_per_split = SPLIT ? (k_blocks + splits - 1) / splits : k_blocks;
+  const int items = tiles * splits;
+  auto item_kblocks = [&](int item) {
+    if constexpr (SPLIT) {
+      const int kb0 = (item / tiles) * kb_per_split;
+      return min(k_blocks, kb0 + kb_per_split) - kb0;
+    } else {
+      return k_blocks;
+    }
+  };
 
   if (warp_idx >= kConsumerThreads / 32) {
     // ================= TMA producer warpgroup =================
     setmaxnreg_dec<40>();
     if (warp_idx == kConsumerThreads / 32 && lane == 0)
-      produce<BN, kStages, A_MN, B_MN>(&tmap_a, &tmap_b, smem, full_bar, empty_bar, tiles, tiles, n_tiles, k_blocks, k_blocks);
+      produce<BN, kStages, A_MN, B_MN>(&tmap_a, &tmap_b, smem, full_bar, empty_bar, items, tiles, n_tiles, k_blocks, kb_per_split);
     return;
   }
 
@@ -584,22 +613,24 @@ gemm_bf16_wgmma_pingpong_kernel(const __grid_constant__ CUtensorMap tmap_a, cons
   // complete: it starts at once. Each wait is at most one phase behind the other warpgroup's arrivals (it arrives once per tile
   // and then waits for this warpgroup's arrival), so a parity wait cannot pass early.
   uint32_t order_phase = wg == 0 ? 1u : 0u;
-  // ring position (k-blocks loaded before) of this warpgroup's next k-block; every tile has k_blocks of them
-  int pos = wg * k_blocks;
+  // ring position (k-blocks loaded before) of this warpgroup's next k-block
+  int pos = wg * item_kblocks(blockIdx.x);
   float acc[2][BN / 2];
-  for (int tile = blockIdx.x + wg * gridDim.x; tile < tiles; tile += 2 * gridDim.x) {
+  for (int item = blockIdx.x + wg * gridDim.x; item < items; item += 2 * gridDim.x) {
+    const int tile = SPLIT ? item % tiles : item;
     const int m_blk = tile / n_tiles, n_blk = tile % n_tiles;
+    const int nkb = item_kblocks(item);
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) {
       acc[0][i] = 0.f;
       acc[1][i] = 0.f;
     }
-    // The other warpgroup has issued every MMA of the previous tile, so it has also seen every k-block before this tile's arrive:
-    // the full_bar slots this tile waits for are at most one phase ahead of what has completed.
+    // The other warpgroup has issued every MMA of the previous item, so it has also seen every k-block before this item's arrive:
+    // the full_bar slots this item waits for are at most one phase ahead of what has completed.
     mbar_wait(&order_bar[wg], order_phase);
     order_phase ^= 1u;
     int prev_stage = pos % kStages;
-    for (int kb = 0; kb < k_blocks; ++kb, ++pos) {
+    for (int kb = 0; kb < nkb; ++kb, ++pos) {
       const int stage = pos % kStages;
       mbar_wait(&full_bar[stage], (uint32_t) (pos / kStages) & 1u);
       const uint32_t a_addr = smem_u32(smem + stage * L::kStageBytes);
@@ -613,15 +644,41 @@ gemm_bf16_wgmma_pingpong_kernel(const __grid_constant__ CUtensorMap tmap_a, cons
       if (kb > 0 && leader) mbar_arrive(&empty_bar[prev_stage]);
       prev_stage = stage;
     }
-    if (leader) mbar_arrive(&order_bar[wg ^ 1]);  // this tile's last MMAs are issued: the other warpgroup's mainloop may start
-    pos += k_blocks;                              // (the other warpgroup's tile)
+    if (leader) mbar_arrive(&order_bar[wg ^ 1]);  // this item's last MMAs are issued: the other warpgroup's mainloop may start
+    pos += item_kblocks(item + gridDim.x);        // (the other warpgroup's item)
     wgmma_wait<0>();
     wgmma_fence_regs(acc[0]);
     wgmma_fence_regs(acc[1]);
     if (leader) mbar_arrive(&empty_bar[prev_stage]);
     const int row0 = m_blk * BLOCK_M, n0 = n_blk * BN;
     // the epilogue runs once per 64-row half, each with its own column-sum scratch (no barrier between the two)
-    if constexpr (TMA_OUT) {
+    if constexpr (SPLIT) {
+      // The partial tile leaves through TMA reduce-adds (performed in L2): the warpgroup returns to its next item's MMAs once they
+      // are committed. The 128 x 128 fp32 tile is twice the staging buffer, so the two 64-row halves take turns in it, each as four
+      // 64 x 32 SWIZZLE_128B boxes (the tensor map clips rows / columns outside the output).
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        if (leader) tma_store_wait_read();  // the previous half's reduce-adds have read the staging buffer
+        warpgroup_sync(wg);
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh) {
+            const int r = 16 * wq + (lane >> 2) + 8 * hh, c = 8 * (j & 3) + 2 * (lane & 3);
+            const float2 v = make_float2(acc[h][4 * j + 2 * hh] * p.alpha, acc[h][4 * j + 2 * hh + 1] * p.alpha);
+            *reinterpret_cast<float2*>(out_stage + (j >> 2) * 8192 + sw128_offset_f32(r, c)) = v;
+          }
+        }
+        fence_proxy_async();
+        warpgroup_sync(wg);
+        if (leader && row0 + 64 * h < p.M) {
+#pragma unroll
+          for (int b = 0; b < BN / 32; ++b)
+            if (n0 + 32 * b < p.N) tma_reduce_add_2d(&tmap_out, out_stage + b * 8192, n0 + 32 * b, row0 + 64 * h);
+          tma_store_commit();
+        }
+      }
+    } else if constexpr (TMA_OUT) {
       if (leader) tma_store_wait_read();  // this warpgroup's previous stores have read the staging buffer
       warpgroup_sync(wg);                 // ... and every warp is past the previous epilogue (colsum_s / bias_s are free as well)
       if (p.bias != nullptr) {
@@ -655,7 +712,7 @@ gemm_bf16_wgmma_pingpong_kernel(const __grid_constant__ CUtensorMap tmap_a, cons
       }
     }
   }
-  if constexpr (TMA_OUT) {
+  if constexpr (TMA_OUT || SPLIT) {
     if (leader) tma_store_wait_all();
   }
 }
@@ -687,6 +744,20 @@ int make_tmap(CUtensorMap* map, const void* ptr, int64_t rows, int64_t K, int64_
   return r == CUDA_SUCCESS ? 0 : -11;
 }
 
+// rows x cols fp32 output of the split-K reduce-adds, row pitch ld elements; box = 32 columns (128 B) x 64 rows, SWIZZLE_128B.
+// The map needs a 16 B aligned base and row pitch.
+int make_tmap_f32_out(CUtensorMap* map, void* ptr, int64_t rows, int64_t cols, int64_t ld) {
+  EncodeTiledFn fn = get_encode_fn();
+  if (fn == nullptr || reinterpret_cast<uintptr_t>(ptr) % 16 != 0 || ld % 4 != 0) return -11;
+  cuuint64_t dims[2] = {(cuuint64_t) cols, (cuuint64_t) rows};
+  cuuint64_t strides[1] = {(cuuint64_t) ld * 4};
+  cuuint32_t box[2] = {32, 64};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                  CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS ? 0 : -11;
+}
+
 template <int BN, bool A_MN, bool B_MN>
 int launch_gemm_persistent(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to, const GemmParams& p, cudaStream_t stream) {
   constexpr int smem_bytes = PersistentLayout<BN>::kTotal + 1024;
@@ -712,17 +783,21 @@ int launch_gemm_pingpong(const CUtensorMap& ta, const CUtensorMap& tb, const CUt
   constexpr int smem_bytes = PingPongLayout::kTotal + 1024;
   static bool configured = false;
   if (!configured) {
-    TRB_CUDA(cudaFuncSetAttribute(gemm_bf16_wgmma_pingpong_kernel<A_MN, B_MN, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
-    TRB_CUDA(cudaFuncSetAttribute(gemm_bf16_wgmma_pingpong_kernel<A_MN, B_MN, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
+    TRB_CUDA(cudaFuncSetAttribute(gemm_bf16_wgmma_pingpong_kernel<A_MN, B_MN, PP_TMA>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
+    TRB_CUDA(cudaFuncSetAttribute(gemm_bf16_wgmma_pingpong_kernel<A_MN, B_MN, PP_DIRECT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
+    TRB_CUDA(cudaFuncSetAttribute(gemm_bf16_wgmma_pingpong_kernel<A_MN, B_MN, PP_ADD_F32>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
     configured = true;
   }
-  const int64_t tiles = (int64_t) ((p.M + BLOCK_M - 1) / BLOCK_M) * ((p.N + PingPongLayout::BN - 1) / PingPongLayout::BN);
-  if (tiles > 0x7fffffff) return -12;
-  const int grid = (int) (tiles < trb_num_sms() ? tiles : trb_num_sms());
-  if (p.tma_out)
-    gemm_bf16_wgmma_pingpong_kernel<A_MN, B_MN, true><<<grid, kPersistentThreads, smem_bytes, stream>>>(ta, tb, to, p);
+  // split-K (fp32 output described by `to`): one item per (tile, K-slice)
+  const int64_t items = (int64_t) ((p.M + BLOCK_M - 1) / BLOCK_M) * ((p.N + PingPongLayout::BN - 1) / PingPongLayout::BN) * p.split_k;
+  if (items > 0x7fffffff) return -12;
+  const int grid = (int) (items < trb_num_sms() ? items : trb_num_sms());
+  if (p.split_k > 1)
+    gemm_bf16_wgmma_pingpong_kernel<A_MN, B_MN, PP_ADD_F32><<<grid, kPersistentThreads, smem_bytes, stream>>>(ta, tb, to, p);
+  else if (p.tma_out)
+    gemm_bf16_wgmma_pingpong_kernel<A_MN, B_MN, PP_TMA><<<grid, kPersistentThreads, smem_bytes, stream>>>(ta, tb, to, p);
   else
-    gemm_bf16_wgmma_pingpong_kernel<A_MN, B_MN, false><<<grid, kPersistentThreads, smem_bytes, stream>>>(ta, tb, to, p);
+    gemm_bf16_wgmma_pingpong_kernel<A_MN, B_MN, PP_DIRECT><<<grid, kPersistentThreads, smem_bytes, stream>>>(ta, tb, to, p);
   TRB_CHECK_LAUNCH();
   return 0;
 }
@@ -764,6 +839,14 @@ static int gemm_dispatch(const void* A, int64_t lda, const void* B, int64_t ldb,
   memset(&to, 0, sizeof(to));
   p.tma_out = !p.out_f32 && p.split_k == 1 && reinterpret_cast<uintptr_t>(p.out) % 16 == 0 && p.ldo % 8 == 0 &&
               make_tmap(&to, p.out, p.M, p.N, p.ldo, 64, 64) == 0;
+  // Split-K fp32 outputs (the weight gradients) on ping-pong items of (128 x 128 tile, K-slice), each partial tile added into the
+  // output by TMA reduce-adds while the other warpgroup multiplies. An output the tensor map cannot describe (base or row pitch not
+  // 16 B aligned) stays on the cooperative kernel, which adds from the fragment layout with fp32 atomics.
+  if (p.split_k > 1 && make_tmap_f32_out(&to, p.out, p.M, p.N, p.ldo) == 0) {
+    rc = B_MN ? make_tmap(&tb, B, p.K, p.N, ldb, 64, 64) : make_tmap(&tb, B, p.N, p.K, ldb, PingPongLayout::BN);
+    if (rc) return rc;
+    return launch_gemm_pingpong<A_MN, B_MN>(ta, tb, to, p, stream);
+  }
   // Ping-pong for bf16 outputs without split-K, except where the cooperative kernel measured faster (H100, DESIGN.md): N <= 128
   // (one 128 x 128 tile per row-block, split over both warpgroups) and a plain MN-major-B product (a dgrad without a ReLU mask),
   // whose bare conversion epilogue gains less from the overlap than 128 x 256 tiles save in operand traffic.

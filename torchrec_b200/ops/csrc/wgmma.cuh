@@ -45,6 +45,13 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, const void*
                ::"l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(smem)), "r"(c0), "r"(c1)
                : "memory");
 }
+// TMA reduce-add of a box from shared memory into global memory (element-wise add performed in L2; same completion and fences
+// as tma_store_2d)
+__device__ __forceinline__ void tma_reduce_add_2d(const CUtensorMap* map, const void* smem, int c0, int c1) {
+  asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(smem)), "r"(c0), "r"(c1)
+               : "memory");
+}
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 // the committed stores have finished reading shared memory (the source may be overwritten)
 __device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }

@@ -34,10 +34,11 @@ def gemm_bf16(a: torch.Tensor, b: torch.Tensor, a_mn: bool = False, b_mn: bool =
               out: Optional[torch.Tensor] = None, split_k: int = 1, tile_n: int = 0, mask_bits: Optional[torch.Tensor] = None,
               relu_bits_out: Optional[torch.Tensor] = None, colsum_ws: Optional[torch.Tensor] = None) -> torch.Tensor:
     """``act(alpha * op(a) @ op(b)^T + bias)`` on the wgmma kernels: 128 x 64 tiles for N <= 64 (two CTAs per SM), otherwise a
-    persistent kernel (one CTA per SM): bf16 outputs without split-K at N > 128 on 128 x 128 tiles, one per consumer warpgroup
-    (ping-pong: one warpgroup's epilogue runs while the other multiplies), unless the product is plain (no bias, activation or column
-    sums) with an MN-major b; otherwise both warpgroups on one tile, 128 x 128 for N <= 128 and 128 x 256 above (128 x 128 for
-    split-K up to N = 256).
+    persistent kernel (one CTA per SM): bf16 outputs without split-K at N > 128, and split-K fp32 outputs with a 16 B aligned base and
+    row pitch, on 128 x 128 tiles, one per consumer warpgroup (ping-pong: one warpgroup's epilogue runs while the other multiplies;
+    split-K partial tiles are added into ``out`` by TMA reduce-adds), unless the product is plain (no bias, activation or column sums)
+    with an MN-major b; otherwise both warpgroups on one tile, 128 x 128 for N <= 128 and 128 x 256 above (128 x 128 for split-K up
+    to N = 256).
     ``tile_n``: the tile width the caller sized ``split_k`` for (a hint; the kernel's tile depends on N and split-K only). ``relu_bits_out`` (int32
     ``[M, ceil(N / 32)]``, with ``ACT_RELU``): receives one bit per output (> 0); ``mask_bits`` (same layout, with ``ACT_RELU_GRAD``): used instead of re-reading ``mask``.
 
@@ -134,7 +135,8 @@ RELU_BITS = os.environ.get("TRB_GEMM_RELU_BITS", "1") != "0"
 
 def _best_split(tiles: int, K: int, sms: int) -> int:
     """Split-K factor that fills whole waves of the grid: maximise tiles*s / (ceil(tiles*s / sms) * sms) over splits that keep
-    >= 512 reduction elements each (fewer, fuller waves beat many splits: every split adds a pass of fp32 atomics)."""
+    >= 512 reduction elements each (fewer, fuller waves beat many splits: every split adds one fp32 partial tile per item to reduce
+    into the output, and one more item start to each CTA's list)."""
     best, best_score = 1, -1.0
     for s in range(1, max(1, min(64, K // 512)) + 1):
         items = tiles * s
@@ -144,14 +146,17 @@ def _best_split(tiles: int, K: int, sms: int) -> int:
     return best
 
 
-# 128 x 128 work items per SM in one wave of the GEMM grid: the persistent kernel (csrc/gemm_wgmma.cu) runs one CTA per SM on 128 x 256
-# tiles, i.e. two 128 x 128 items, and the 128 x 64 kernel of N <= 64 runs two CTAs per SM
+# 128 x 128 work items per SM in one wave of the split-K GEMM grid: the ping-pong kernel (csrc/gemm_wgmma.cu) runs one CTA per SM whose
+# two consumer warpgroups each own one (tile, K-slice) item at a time, and the 128 x 64 kernel of N <= 64 runs two CTAs per SM. Two
+# items per CTA let the first item's reduce-add epilogue run under the second one's MMAs; a multiple of 2 x SMs items also keeps every
+# CTA's list, and so its tensor-core time, the same length (see _best_split)
 GEMM_CTAS_PER_SM = 2
 
 
 def _wgrad_plan(n_out: int, n_in: int, batch: int, sms: int) -> "tuple[int, int]":
     """(split_k, tile_n) of the weight-gradient GEMM ``[n_out, n_in] = gy^T[n_out, batch] . x[batch, n_in]``, sized in 128 x 128 items
-    (GEMM_CTAS_PER_SM x SMs of them fill one wave, also when the kernel runs them as 128 x 256 tiles)."""
+    (GEMM_CTAS_PER_SM x SMs of them fill one wave). At batch 32768 on 132 SMs the DLRM step's wgrads get 256 or 264 items: two per
+    CTA, one per consumer warpgroup, on all but at most 8 CTAs."""
     tiles = ((n_out + 127) // 128) * ((n_in + 127) // 128)
     return _best_split(tiles, batch, GEMM_CTAS_PER_SM * sms), 128
 
